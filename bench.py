@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- SoftRas forward+backward throughput on B200 (BASELINE.json metric).
+"""bench.py -- SoftRas forward+backward throughput on one or more GPUs (BASELINE.json metric).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload c3|c2|tiny]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload c3|c2|tiny] [--dump-outputs DIR]
     (N>1: python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...)
 
 Workload (default "c3", BASELINE.json configs[2] / the README's 39k-face row): UV sphere with
@@ -11,9 +11,16 @@ euclidean / softmax / prod, K=16), 4 images per GPU -- B=32 at 8 GPUs, weak scal
 
 Prints ONE JSON line (rank 0).  `value` = frames/s over all ranks with inputs resident in
 HBM; `e2e` = same through the public API with pinned HOST inputs, H2D/D2H inside the timed
-region; `roofline` = the dominant kernel against the measured HBM peak; `cpu_baseline` =
+region; `roofline` = the dominant kernel against the HBM peak; `cpu_baseline` =
 the CPU oracle (restatement of the reference kernels; the reference has no CPU path,
-SURVEY.md F1) on this box's host cores on a bounded sample.
+SURVEY.md F1) on the host's cores on a bounded sample.
+
+--dump-outputs DIR writes, after the timed steps, what the last timed step computed as DIR/<name>.npy (float32):
+for SoftRas the RGBA images and the gradients of face_vertices and textures, for NMR (c4) the RGB images and the
+gradients of faces and textures, for c1 the last rendered RGB view, for c5 the silhouettes of the last iteration and
+the fitted mesh vertices (of the faster of the eager and CUDA-graph runs).  An array larger than 32 MiB is written as a fixed sample: the values at
+DUMP_SAMPLE flat positions drawn with numpy.random.default_rng(0).choice(size, DUMP_SAMPLE, replace=False), sorted.
+The inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -46,6 +53,9 @@ WORKLOADS = {
 }
 ASSETS = os.path.join(ROOT, "baseline", "_ref", "assets", "data")   # staged by tools/stage_assets.py where /root/reference exists
 README_39K_MS = 35.5  # BASELINE.md section 1: Jrender SoftRas 39k faces, 1024^2, hardware/batch unstated
+HBM_GBS_DATASHEET = 3350.0   # H100 SXM data sheet HBM3 bandwidth (700 W card)
+DUMP_LIMIT = 32 << 20        # bytes per dumped array before it is sampled (c3 dumps 24 MiB in all, c4 48 MiB)
+DUMP_SAMPLE = 1 << 22        # float32 values kept of a sampled array (16 MiB)
 
 
 def parse_args():
@@ -60,6 +70,8 @@ def parse_args():
     ap.add_argument("--option", action="append", default=[], metavar="NAME=VALUE",
                     help="b200r_set_option() knob for A/B runs, e.g. --option softras_exact_tail=1")
     ap.add_argument("--cpu-seconds", type=float, default=15.0, help="target CPU-baseline sample time")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32, sampled above 32 MiB)")
     return ap.parse_args()
 
 
@@ -70,7 +82,19 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return HBM_GBS_DATASHEET, "H100 SXM data sheet (3.35 TB/s), not measured"
+
+
+def dump_outputs(directory, arrays):
+    """Writes {name: tensor or ndarray} as DIR/<name>.npy in float32; arrays above DUMP_LIMIT as the seeded sample
+    described in the module docstring."""
+    os.makedirs(directory, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a.detach().float().cpu().numpy() if hasattr(a, "detach") else a, dtype=np.float32)
+        if a.nbytes > DUMP_LIMIT:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, DUMP_SAMPLE, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(directory, name + ".npy"), a)
 
 
 def build_inputs(workload, rank, world):
@@ -87,7 +111,7 @@ def build_inputs(workload, rank, world):
 
 # --------------------------------------------------------------------------- clocks
 class ClockSampler:
-    """nvidia-smi sampler running DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampler running DURING the timed region (SM clock, power draw, throttle reasons)."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -230,7 +254,7 @@ def run_ours(args, rank, world, local_rank):
     fv = torch.from_numpy(fv_h).to(dev).requires_grad_(True)
     tex = torch.from_numpy(tex_h).to(dev).requires_grad_(True)
     grad = torch.from_numpy(grad_h).to(dev)
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # 256 MiB > the 50 MB L2
 
     def step():
         fv.grad = None
@@ -256,14 +280,19 @@ def run_ours(args, rank, world, local_rank):
     launches0 = L.b200r_launch_count()
     ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
     barrier()
+    img = None
     for a, b in ev:
+        img = None                # the previous step's output is released before the next step, as in the warm-up
         flush.fill_(1.0)          # L2 flush between timed iterations (outside the event pair)
         a.record()
-        step()
+        img = step()
         b.record()
     barrier()
     launches = L.b200r_launch_count() - launches0
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"soft_colors": img, "grad_face_vertices": fv.grad, "grad_textures": tex.grad})
+    del img
     step_ms = [a.elapsed_time(b) for a, b in ev]
     t_rank = torch.tensor([sum(step_ms)], dtype=torch.float64, device=dev)
     if world > 1:
@@ -508,10 +537,10 @@ def run_ours(args, rank, world, local_rank):
         gather_steps = {"images_identical": same, "step_no_gather_ms": t_plain, "step_blocking_gather_ms": timed(step_blocking),
                         "step_overlapped_gather_ms": {"chunk_%d_images" % c: timed(f) for c, f in overlapped.items()},
                         "step_pipelined_gather_ms": timed(step_pipelined),
-                        "note": "each includes a 256 MiB L2 flush write per step (~0.08 ms), unlike ms_per_step; chunk = images per "
+                        "note": "each includes a 256 MiB L2 flush write per step, unlike ms_per_step; chunk = images per "
                                 "forward launch (chunk == images_per_gpu: one launch, the gather hides behind the backward; smaller "
                                 "chunks hide it behind the next chunk's raster too but every launch is bound by the serial chain of its pole "
-                                "blocks, ~0.8 ms whatever the number of images in it); pipelined = the "
+                                "blocks whatever the number of images in it); pipelined = the "
                                 "batch of step n is collected during step n+1, behind its own backward and the next raster"}
         pipe["pending"].result()
 
@@ -526,28 +555,6 @@ def run_ours(args, rank, world, local_rank):
     dom = max(alg, key=lambda k: kern[k]["avg_ms"])
     peak, peak_src = peaks()
     achieved = alg[dom] / (kern[dom]["avg_ms"] / 1000.0) / 1e9
-    traffic = None   # measured DRAM bytes per launch of the dominant kernel, from the committed ncu capture
-    try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "ncu_traffic.json")) as f:
-            traffic = json.load(f).get(args.workload, {}).get(dom)
-    except OSError:
-        pass
-    # Secondary, more telling figure for this SIMT-bound path: warp instructions per launch (from the committed ncu
-    # capture) over the measured kernel time, against the SM's issue ceiling (SMs x 4 schedulers x SM clock).
-    issue = None
-    try:
-        with open(os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "ncu_traffic.json")) as f:
-            ninst = json.load(f).get(args.workload + "_warp_instructions", {}).get(dom)
-        if ninst and clocks and clocks.get("sm_mhz"):
-            import torch as _t
-            sms = _t.cuda.get_device_properties(dev).multi_processor_count
-            peak_i = sms * 4 * clocks["sm_mhz"] * 1e6
-            ach_i = ninst / (kern[dom]["avg_ms"] / 1000.0)
-            issue = {"kernel": dom, "warp_instructions_per_launch": int(ninst), "achieved_ginst_s": ach_i / 1e9,
-                     "peak_ginst_s": peak_i / 1e9, "frac": ach_i / peak_i,
-                     "note": "instruction count from the committed ncu capture (profiles/), time measured live"}
-    except Exception:
-        issue = None
     step_alg = bpg * (48 * P + 3 * (36 + 12 * T) * nf)
     line = {
         "metric": METRIC, "value": value, "unit": "frames/s", "n_gpus": world, "steps": args.steps,
@@ -563,15 +570,13 @@ def run_ours(args, rank, world, local_rank):
         "gpu_launches": int(launches),
         "kernels": kern,
         "roofline": {"bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                     "frac": achieved / peak, "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": int(alg[dom]),
-                     "note": "SIMT fp32 rasterization is issue-bound, not HBM-bound (SURVEY.md F9); see profiles/"},
+                     "note": "SIMT fp32 rasterization is issue-bound, not HBM-bound (SURVEY.md F9)"},
         "roofline_step": {"algorithmic_bytes_per_step": int(step_alg),
                           "achieved_gbs": step_alg / (total_ms / args.steps / 1000.0) / 1e9,
                           "frac": step_alg / (total_ms / args.steps / 1000.0) / 1e9 / peak},
     }
-    if issue is not None:
-        line["roofline_issue"] = issue
     if gather_ms is not None:
         line["allgather_images_ms"] = gather_ms
         line["gather_in_step"] = gather_steps
@@ -607,7 +612,7 @@ def run_nmr(args, rank, world, local_rank):
     tex_h = np.ascontiguousarray(np.repeat(tex_h, bpg, 0))
     faces = torch.from_numpy(faces_h).to(dev).requires_grad_(True)
     tex = torch.from_numpy(tex_h).to(dev).requires_grad_(True)
-    g = torch.rand((bpg, H, H, 3), device=dev) * 2 - 1
+    g = torch.from_numpy(np.random.default_rng(3 + rank).uniform(-1.0, 1.0, (bpg, H, H, 3)).astype(np.float32)).to(dev)
     flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)
 
     def step():
@@ -615,16 +620,22 @@ def run_nmr(args, rank, world, local_rank):
         tex.grad = None
         rgb, _, _ = RasterizeFunction(H, 0.1, 100.0, 1e-3, (0, 0, 0), True, False, False)(faces, tex)
         rgb.backward(g)
+        return rgb
     for _ in range(max(3, args.warmup)):
         step()
     torch.cuda.synchronize(dev)
     ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.steps)]
     l0 = L.b200r_launch_count()
+    rgb = None
     for a, b in ev:
+        rgb = None
         flush.fill_(1.0)
-        a.record(); step(); b.record()
+        a.record(); rgb = step(); b.record()
     torch.cuda.synchronize(dev)
     launches = L.b200r_launch_count() - l0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"rgb": rgb, "grad_faces": faces.grad, "grad_textures": tex.grad})
+    del rgb
     ms = [a.elapsed_time(b) for a, b in ev]
     L.b200r_profile_reset(); L.b200r_profile_enable(1)
     for _ in range(3):
@@ -668,8 +679,8 @@ def run_deform(args, rank, world, local_rank):
     torch.cuda.set_device(dev)
     L = _lib.lib()
     nf, H, views, desc = WORKLOADS["c5"]
-    iters = max(8, args.steps)
     out = {}
+    fitted = {}
     src = {}
     staged = all(os.path.exists(os.path.join(ASSETS, f)) for f in ("source.npy", "camera.npy", "obj/sphere/sphere_1352.obj"))
     if staged:   # demo2-deform.py:50-55 literally: sphere_1352.obj template, data/source.npy silhouettes (64^2, nearest-upsampled), data/camera.npy
@@ -678,17 +689,24 @@ def run_deform(args, rank, world, local_rank):
         desc = "C5: demo2-deform as configured (sphere_1352.obj -> data/source.npy silhouettes, data/camera.npy), 512x512, 120 views/iteration"
     for mode in ("eager", "cuda_graph"):
         l0 = L.b200r_launch_count()
+        # eager: every iteration is timed; cuda_graph: 3 warm-up iterations and the capture come first, untimed
+        iters = args.steps + (4 if mode == "cuda_graph" else 0)
         r = demo2_deform.run(iters=iters, image_size=H, batch_size=views, verbose=False, cuda_graph=(mode == "cuda_graph"),
                              device=str(dev), **src)
         out[mode] = {"ms_per_iter": r["device_ms_per_iter"], "host_ms_per_iter": r["ms_per_iter"], "first_iou": r["first_iou"],
                      "final_iou": r["final_iou"], "library_launches": int(L.b200r_launch_count() - l0),
                      "iou_history": [[int(i), round(float(v), 4)] for i, _, v in r["history"]]}
+        fitted[mode] = {"silhouettes": r["images"], "vertices": r["vertices"]}
     if rank != 0:
         return
-    best = min(out.values(), key=lambda d: d["ms_per_iter"])
+    best_mode = min(out, key=lambda m: out[m]["ms_per_iter"])
+    best = out[best_mode]
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, fitted[best_mode])
     print(json.dumps({
         "metric": "demo2_deform_views_per_s_512px", "value": views * 1000.0 / best["ms_per_iter"], "unit": "frames/s",
-        "n_gpus": world, "steps": iters, "warmup": 3, "ms_per_step": best["ms_per_iter"], "higher_is_better": True,
+        "n_gpus": world, "steps": args.steps, "warmup": 4 if best_mode == "cuda_graph" else 0, "ms_per_step": best["ms_per_iter"],
+        "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "f32",
         "data": "reference assets (baseline/_ref/assets)" if staged else "synthetic",
         "config": {"workload": desc, "optimizer": "Adam(0.01, betas=(0.5, 0.99))", "sigma_val": 1e-4, "mode": "silhouettes"},
@@ -733,6 +751,8 @@ def run_render(args, rank, world, local_rank):
         a.record(); frame(4.0 * k); b.record()
     torch.cuda.synchronize(dev)
     wall = time.perf_counter() - t0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"rgb": host})
     launches = L.b200r_launch_count() - l0
     ms = [a.elapsed_time(b) for a, b in ev]
     L.b200r_profile_reset(); L.b200r_profile_enable(1)

@@ -99,7 +99,10 @@ def run(iters=200, image_size=64, batch_size=24, filename_input=None, camera_inp
         optimizer.step()
         return loss, images_pred
 
+    last = {}
+
     def log(i, loss, images_pred):
+        last["images"] = images_pred.detach()
         if i % 20 == 0 or i == iters - 1:
             hist.append((i, float(loss.item()), iou(images_pred.detach(), target)))
             if verbose:
@@ -144,7 +147,10 @@ def run(iters=200, image_size=64, batch_size=24, filename_input=None, camera_inp
     if output_dir:
         os.makedirs(output_dir, exist_ok=True)
         jr.save_obj(os.path.join(output_dir, 'plane.obj'), model(1)[0].vertices[0], model.faces[0])
-    return dict(ms_per_iter=1000.0 * dt / iters, device_ms_per_iter=1000.0 * dt_dev / iters, batch_size=batch_size, history=hist, final_iou=hist[-1][2], first_iou=hist[0][2])
+    with torch.no_grad():
+        vertices = model(1)[0].vertices[0].detach()
+    return dict(ms_per_iter=1000.0 * dt / iters, device_ms_per_iter=1000.0 * dt_dev / iters, batch_size=batch_size, history=hist, final_iou=hist[-1][2], first_iou=hist[0][2],
+                images=last["images"], vertices=vertices)
 
 
 if __name__ == '__main__':

@@ -1,5 +1,5 @@
 /*
- * b200raster.h -- C ABI of libb200raster.so, the B200 (sm_100a) differentiable
+ * b200raster.h -- C ABI of libb200raster.so, the H100 (sm_90a) differentiable
  * mesh rasterizer that drops in behind Jittor/jrender's rasterizer Functions.
  *
  * Every entry point replaces one `jt.code(...)` op of the reference (paths are

@@ -1,6 +1,6 @@
-"""jrender_b200 -- B200-native differentiable mesh rasterizer behind Jittor/jrender's API.
+"""jrender_b200 -- H100-native differentiable mesh rasterizer behind Jittor/jrender's API.
 
-Hot path: hand-written sm_100a CUDA kernels in csrc/, exposed through the C ABI in
+Hot path: hand-written sm_90a CUDA kernels in csrc/, exposed through the C ABI in
 include/b200raster.h (libb200raster.so) and bound with ctypes; PyTorch is plumbing only
 (device memory, streams, autograd glue) plus the O(nf) host-side mirror of the reference's
 camera / lighting / mesh / loss classes so that reference scripts port by changing the import.

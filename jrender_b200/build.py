@@ -1,8 +1,8 @@
-"""In-tree build of libb200raster.so (hand-written sm_100a CUDA, C ABI in include/b200raster.h).
+"""In-tree build of libb200raster.so (hand-written sm_90a CUDA, C ABI in include/b200raster.h).
 
     python -m jrender_b200.build [--force] [--verbose]
 
-Flags: -gencode arch=compute_100a,code=sm_100a (B200 only), -lineinfo (ncu source view),
+Flags: -gencode arch=compute_90a,code=sm_90a (H100 / Hopper only), -lineinfo (ncu source view),
 -fmad=false (no a*b+c contraction: see csrc/common.cuh for the arithmetic contract; IEEE
 division / sqrt are nvcc defaults and must not be weakened -- no --use_fast_math).
 """
@@ -16,7 +16,7 @@ LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libb200raster.so")
 SOURCES = ["softras_api.cu", "softras_fwd.cu", "softras_bwd.cu",
            "nmr_api.cu", "preraster_api.cu", "mesh_loss_api.cu", "lighting_api.cu", "bake_api.cu", "api_util.cu", "debug_api.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-fmad=false", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
 OBJDIR = os.path.join(HERE, "lib", "obj")
 

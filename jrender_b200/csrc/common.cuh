@@ -1,4 +1,4 @@
-// common.cuh -- shared definitions of the B200 rasterizer kernels.
+// common.cuh -- shared definitions of the rasterizer kernels.
 //
 // Arithmetic contract: this translation unit set is compiled with -fmad=false
 // (no a*b+c contraction), IEEE division and sqrt (nvcc defaults -prec-div=true,

@@ -8,7 +8,7 @@
 //   K10 backward_textures_cuda_kernel        :659-694
 //   K11 backward_depth_map_cuda_kernel       :738-788
 //
-// B200 design: the forward is a face-parallel z-buffer pass (a warp per face over its bounding box, one 64-bit atomicMin
+// Design: the forward is a face-parallel z-buffer pass (a warp per face over its bounding box, one 64-bit atomicMin
 // of (depth, face id) per covered pixel: lock-free and deterministic -- lowest face id wins equal depth; the reference's
 // winner is race-dependent) followed by a per-pixel resolve pass that fuses K7's map writes with K8: the pixel recomputes
 // its winning face's weights, samples the texture and writes every map once.  K9 keeps the reference's per-face edge walk but gives a WARP to each
@@ -117,7 +117,7 @@ __device__ __forceinline__ uint32_t nmr_order_bits(float z) {
 // K7, pass 1 -- face-parallel z-buffer.  The reference gives a THREAD to every face and serialises pixels behind an
 // atomicCAS spin lock (:138-160, the winner of equal depths is whoever gets the lock first); the first version here was
 // tile-centric (every pixel of a 16x16 tile tested every face binned to the tile: ~100 bounding-box tests per pixel for
-// the 2-pixel triangles of the 39 200-face mesh, 1.1 ms + 0.3 ms of binning per 16 images).  Now every covered pixel of
+// the 2-pixel triangles of the 39 200-face mesh, plus a binning pass).  Now every covered pixel of
 // every face does ONE 64-bit atomicMin of (depth order bits << 32 | face id) into the z-buffer: lock-free, and
 // deterministic -- lowest depth, then lowest face id, exactly the oracle's tie rule.  A thread sets its face up and walks a
 // small bounding box itself (the per-face set-up with its nine divisions is most of the work for small faces: 32 faces
@@ -418,7 +418,7 @@ __device__ __forceinline__ void k9_scan(const float* __restrict__ prow, const in
 //  * delta advances by 64 per trip instead of being re-formed from the pixel number (<= 1 ulp of delta).
 //  * Two records per lane in flight, ping-pong: the load of trip t + 2 is issued as soon as trip t's record has been
 //    consumed and is only needed after trip t + 1's arithmetic -- the generic loop below re-used the record's registers
-//    and waited for every load (long_scoreboard 8.1 per issue in profiles/r02d).
+//    and waited for every load (long-scoreboard stalls dominated).
 // Trip count is warp-uniform; only the loads are predicated.
 template <int MODE>
 struct K9Px { float4 q; float ga; };
@@ -516,7 +516,8 @@ __device__ __forceinline__ K9Pass k9_pass(int pass, const float px[3], const flo
 // lanes have pixels to work on.  d1_cross / d0_cross2 -- which pick pixels through floor / ceil -- keep the reference's
 // exact, unfused arithmetic; the per-sample quotients that only scale `dist` use the approximate reciprocal.
 #ifndef B200R_K9_MINB
-#define B200R_K9_MINB 6   // resident 256-thread CTAs per SM (40 registers: 4.46 ms at C4 against 4.96 at 5 and 5.02 at 4 -- the scans are latency-bound)
+#define B200R_K9_MINB 3   // resident 256-thread CTAs per SM (80 registers, no spills).  H100, C4: 4.51 ms at 3,
+                          // 4.70 at 2 (128 registers), 4.55 at 4 (64, spills), 5.14 at 5, 5.55 at 6, 6.23 at 8 -- the scans are latency-bound
 #endif
 template <int MODE>
 __global__ void __launch_bounds__(256, B200R_K9_MINB)
@@ -607,7 +608,7 @@ k_nmr_backward_pixel_map(const float* __restrict__ faces, const int* __restrict_
         if (!live) { in_from = 1; in_to = 0; }
         // ---- inward scans of small faces: a few pixels each, so every lane walks ITS OWN sample's pixels (:556-601) instead
         // of the warp visiting the samples one after the other for a single partly filled trip each.  (Requesting a pixel's
-        // record together with its owner, instead of after the owner test, was slower: 3.30 vs 3.18 ms at C4.)
+        // record together with its owner, instead of after the owner test, was slower at C4.)
         constexpr int kSerialIn = 64;
         if (in_from <= in_to && in_to - in_from < kSerialIn) {
             const float* __restrict__ prow_l = ((axis == 0) ? pv_img : ph_img) + d0 * is * FL;

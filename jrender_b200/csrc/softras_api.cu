@@ -57,7 +57,7 @@ SoftRasParams make_params(int B, int nf, int T, int is, int K, float near_, floa
 
 extern "C" {
 
-const char* b200r_version(void) { return "b200raster 0.1 (sm_100a)"; }
+const char* b200r_version(void) { return "b200raster 0.1 (sm_90a)"; }
 
 int b200r_set_option(const char* name, int value) {
     if (!name) return b200r_fail(B200R_EINVAL, "b200r_set_option: NULL name");

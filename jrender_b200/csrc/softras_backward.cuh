@@ -11,8 +11,8 @@
 //    [.,9] and grad_textures [.,1,3] (36-byte rows cannot take 16-byte atomics directly).
 //    Atomic packets drop 4x against the reference and no zero-fill of the outputs is needed.
 //    (A walk in ascending face id -- ids staged and sorted in shared memory so that neighbouring lanes sit on the
-//    same record at the same step -- was measured and dropped: 0.518 vs 0.482 ms at C3; the sort costs more
-//    than the L1 sectors it saves.)
+//    same record at the same step -- was measured and dropped: slower at C3; the sort costs more than the L1
+//    sectors it saves.)
 //  VARIANT 0 "warp union walk": every lane sorts its ids ascending and the warp walks the UNION
 //    of its lanes' ids (redux.sync min picks the next face); holders compute, a shuffle tree
 //    sums the 12 values and one lane issues scalar atomics: one set per (warp, face).
@@ -26,13 +26,12 @@
 #ifndef B200R_BWD_MERGE
 #define B200R_BWD_MERGE 1        // warp-side aggregation levels before the atomics: 0 off, 1 = lanes ^1 and ^8, 2 = also ^2 and ^16
                                  // (a complete per-face reduction -- match.any groups + block-floating-point REDUX.SUM --
-                                 // was measured at 1.73 ms against 0.44 ms at C3: profiles/perf_r02.md)
+                                 // was measured at several times the time of level 1 at C3)
 #endif
 #ifndef B200R_BWD_MINB
-// resident 256-thread CTAs per SM the backward's register allocation must allow.  Measured at C3: 2 (107 registers)
-// 0.571 ms, 3 (80) 0.481 ms, 4 (64, 16 B spilled) 0.483 ms -- past 24 warps/SM the kernel is bound by the divergent
-// 160-byte record gathers (L1 throughput 66 %), not by latency; at C5 (3 280 large faces, 60 views) all three give
-// 0.77 ms: there the float atomics on a few thousand hot accumulator rows are the limit.
+// resident 256-thread CTAs per SM the backward's register allocation must allow.  Measured on the H100 at C3: 2 -> 0.675 ms,
+// 3 -> 0.606 ms, 4 -> 0.638 ms -- past 24 warps/SM the divergent 160-byte record gathers and the float atomics bind, not
+// latency.
 #define B200R_BWD_MINB 3
 #endif
 #ifndef B200R_BWD_OPTIMISTIC
@@ -290,7 +289,7 @@ k_softras_backward_lane(const SoftRasParams P, const FaceRec* __restrict__ recs,
 
     // ids are fetched two slots ahead, so the id of the NEXT face is already in a register when
     // its record is prefetched (waiting for a just-issued id load here stalled every iteration).
-    // Prefetching two pairs ahead (ids three ahead) was measured too: no gain (0.487 vs 0.480 ms at C3).
+    // Prefetching two pairs ahead (ids three ahead) was measured too: no gain at C3.
     const bool merge_ok = MERGE && (tex_in_acc || RGB == 2);   // texel-indexed texture gradients are not merged
     int fn_next = (1 < K && has_list) ? __ldg(src + npix) : -1;
     for (int m = 0; m < K; m++) {

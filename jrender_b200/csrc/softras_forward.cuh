@@ -33,7 +33,9 @@ struct __align__(16) FaceRecS {
 #define B200R_FWD_TMA 0       // 1: records staged by cp.async.bulk (TMA) + mbarrier instead of LDG -> registers -> STS
 #endif
 #ifndef B200R_FWD_MINB1
-#define B200R_FWD_MINB1 24    // resident one-warp CTAs per SM the register allocation must allow (80 registers)
+#define B200R_FWD_MINB1 20    // resident one-warp CTAs per SM the register allocation must allow (96 registers).  H100, C3:
+                              // forward 1.08 ms at 20, 1.10 at 16, 1.29 at 24.  Spills (ptxas, sm_90a): the C3 instantiation
+                              // <2,1,false> 144 B stored / 272 B loaded at 96 registers (304 / 584 B at 80); the others 0-112 B
 #endif
 
 // ---- mbarrier / bulk-copy (TMA) helpers ------------------------------------------------------------------------

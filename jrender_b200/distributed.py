@@ -50,8 +50,7 @@ def all_gather_images(images, batch_size=None):
 
 class OverlappedImageGather:
     """The optional all-gather of the output images on a side stream, so that it hides behind whatever the caller
-    enqueues next (the backward pass; with `chunk` < images_per_rank also the rasterization of the following chunks):
-    at C3 the blocking gather is 0.18 / 0.8 ms of a 1.4 ms step on 2 / 8 GPUs.
+    enqueues next (the backward pass; with `chunk` < images_per_rank also the rasterization of the following chunks).
 
         g = OverlappedImageGather(images_per_rank=4, image_shape=(4, 1024, 1024), device=dev)   # chunk = 4: one push
         img = rasterize(batch)                      # [4, 4, H, W] on the current stream
@@ -59,9 +58,9 @@ class OverlappedImageGather:
         loss.backward()                             # ... runs while the gather is in flight
         full = g.result()                           # [world * 4, 4, H, W]; the current stream waits for the side stream
 
-    One launch for the whole batch is the fast configuration (2 GPUs: 1.44 ms per step against 1.40 without and 1.58 with
-    a blocking gather); chunk = 1 or 2 was slower (2.2 / 3.6 ms): a forward launch at this mesh is bound by the serial chain
-    of its heaviest blocks (~0.8 ms) however few images it holds, so splitting the batch multiplies that (DESIGN.md section 4).
+    One launch for the whole batch is the fast configuration; chunk = 1 or 2 was slower: a forward launch at this mesh is
+    bound by the serial chain of its heaviest blocks however few images it holds, so splitting the batch multiplies that
+    (DESIGN.md section 4).
 
     Sample r * images_per_rank + i of the result is chunk i of rank r, i.e. the same order all_gather_images gives.
     Equal shards only.  On CPU tensors (gloo, tests) the calls run synchronously.  Without a process group the result
@@ -98,7 +97,7 @@ class OverlappedImageGather:
                 self.out[:, lo:lo + self.chunk].copy_(dst.view((self.world, self.chunk) + tuple(self.out.shape[2:])))
             return
         # No Tensor.record_stream here: a recorded block makes the caching allocator poll events on every later
-        # allocation and grow the pool while they are pending (measured: 4.3 ms per C3 step instead of 1.47).  Holding
+        # allocation and grow the pool while they are pending (measured: the C3 step took about three times as long).  Holding
         # the reference until result() -- after which the current stream has waited for the side stream -- is enough.
         self._keep.append(src)
         self.side.wait_stream(torch.cuda.current_stream(self.device))

@@ -6,7 +6,7 @@ Mirrors (same names, arguments, defaults, return conventions):
   jrender/renderer/dr/n3mr/n3mr.py:189-346     rasterize_rgbad / rasterize / rasterize_silhouettes / rasterize_depth
   jrender/renderer/dr/n3mr/rasterizer.py:9-105 vertices_to_faces, N3mrRasterizer
 
-Compute: libb200raster.so (b200r_nmr_forward / b200r_nmr_backward, hand-written sm_100a
+Compute: libb200raster.so (b200r_nmr_forward / b200r_nmr_backward, hand-written sm_90a
 kernels); PyTorch owns memory, the stream and autograd glue.  CUDA tensors only.
 """
 import ctypes as C

@@ -5,7 +5,7 @@ Mirrors (same names, argument meaning, defaults and error behaviour):
   jrender/renderer/dr/softras/soft_rasterize.py:136-148 soft_rasterize
   jrender/renderer/dr/softras/rasterizer.py:8-61        SoftRasterizer
 
-The compute is done by libb200raster.so (hand-written sm_100a kernels) through the C ABI
+The compute is done by libb200raster.so (hand-written sm_90a kernels) through the C ABI
 in include/b200raster.h; PyTorch only owns device memory, the stream and autograd glue.
 There is no CPU path: tensors must live on a CUDA device.
 """

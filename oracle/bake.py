@@ -2,7 +2,7 @@
 
 numpy restatement of load_textures_cuda_kernel, jrender/io/utils/load_textures.py:11-69 (barycentric sample point per
 texel :29-37, UV -> image position :42-45, bilinear fetch :46-58, same float / double promotions).  Pinned against the
-reference's own kernel compiled from /root/reference (oracle/build_ref.py) and run on a B200:
+reference's own kernel compiled by oracle/build_ref.py and run on a GPU (named in the file's provenance):
 tests/golden/ref_gpu_bake_random40_R5.npz (generator oracle/make_ref_golden.py --bake-only).
 """
 import numpy as np
@@ -58,7 +58,7 @@ def bake_textures_for_n3mr(image, faces_uv, textures, is_update, texture_wrappin
     image [H,W,3] (already flipped vertically by the caller), faces_uv [nf,3,2], textures [nf,ts,ts,ts,3] (returned updated
     where is_update != 0).  The reference wraps the face's UVs in place from all of the face's threads (a race); like the
     product, every texel here wraps the original UVs once.  Pinned against the reference's own kernel compiled from
-    /root/reference (oracle/build_ref.py) and run on a B200: tests/golden/ref_gpu_bake_n3mr_*.npz
+    the reference (oracle/build_ref.py) and run on a GPU (named in each file's provenance): tests/golden/ref_gpu_bake_n3mr_*.npz
     (generator oracle/make_ref_golden.py --bake-only; its UVs avoid the race's non-fixed points)."""
     nf, ts = textures.shape[0], textures.shape[1]
     assert ts >= 2

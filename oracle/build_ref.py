@@ -5,13 +5,14 @@ and needs Jittor to JIT them; Jittor is not installable here.  This recipe reads
 where they lie under /root/reference (never copied into this repo), captures the `cuda_header`
 strings through a stub `jittor` module, writes them -- plus a small hand-written launcher that
 restates each op's `cuda_src` (memsets, grid/block sizes, argument order) -- to oracle/_ref/*.cu
-and compiles them for sm_100a with nvcc defaults (fmad on, as a stock nvcc/Jittor build would).
+and compiles them for sm_90a with nvcc defaults (fmad on, as a stock nvcc/Jittor build would).
 
     python -m oracle.build_ref
 
 Outputs only into oracle/_ref/ (git-ignored, but shipped to the GPU box by gpurun).  Used to
-(a) generate golden vectors from the real reference kernels on a B200 (oracle/make_ref_golden.py),
-(b) cross-check the product kernels on the GPU, (c) time "the reference kernels on the same B200".
+(a) generate golden vectors from the real reference kernels on the GPU (oracle/make_ref_golden.py,
+oracle/make_ref_parity_golden.py),
+(b) cross-check the product kernels on the GPU, (c) time "the reference kernels on the same GPU".
 """
 import os
 import subprocess
@@ -349,7 +350,7 @@ def build(force=False, verbose=False):
     paths = generate()
     if not force and os.path.exists(LIB) and all(os.path.getmtime(p) <= os.path.getmtime(LIB) for p in paths + [os.path.abspath(__file__)]):
         return LIB
-    cmd = ["/usr/local/cuda/bin/nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    cmd = ["/usr/local/cuda/bin/nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
            "-w", "-Xcompiler", "-fPIC", "-shared", "-o", LIB] + paths
     if verbose:
         print(" ".join(cmd))

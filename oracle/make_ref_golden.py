@@ -89,7 +89,7 @@ def nmr_main(out_dir, report):
         save = dict(faces=faces, textures=tex, grad_rgb_map=grads[0], grad_alpha_map=grads[1], grad_depth_map=grads[2],
                     params=json.dumps(kw),
                     provenance=json.dumps(dict(gpu=torch.cuda.get_device_name(0),
-                                               nvcc="12.9 -O3 -gencode arch=compute_100a,code=sm_100a (fmad default on)",
+                                               nvcc="12.9 -O3 -gencode arch=compute_90a,code=sm_90a (fmad default on)",
                                                source="jrender/renderer/dr/n3mr/cuda/rasterize.py kernels via oracle/build_ref.py")))
         for k, v in ref.items():
             if k in ("alpha_map", "rgb_raw"):
@@ -208,7 +208,7 @@ def main():
             params=json.dumps(dict(P)), soft_colors=ref["soft_colors"], aggrs_info=ref["aggrs_info"],
             faces_id_buffer=ids_ref.astype(np.int16), faces_info=ref["faces_info"],
             grad_faces=ref["grad_faces"], grad_textures=ref["grad_textures"],
-            provenance=json.dumps(dict(gpu=torch.cuda.get_device_name(0), nvcc="12.9 -O3 -gencode arch=compute_100a,code=sm_100a (fmad default on)",
+            provenance=json.dumps(dict(gpu=torch.cuda.get_device_name(0), nvcc="12.9 -O3 -gencode arch=compute_90a,code=sm_90a (fmad default on)",
                                        source="jrender/renderer/dr/softras/cuda/soft_rasterize.py kernels via oracle/build_ref.py")))
         r = dict(name=name)
         r["ids_equal_px_frac"] = float((np.sort(ids_ref, 1) == np.sort(cpu["faces_id_buffer"], 1)).all(1).mean())

@@ -71,7 +71,7 @@ def softras(args):
     if "naive_fwd_ms" in out:
         out["step_ms_naive"] = out["naive_fwd_ms"] + out["bwd_ms"]
         out["frames_per_s_naive"] = B * 1e3 / out["step_ms_naive"]
-    out["what"] = ("reference kernel strings compiled with nvcc -O3 for sm_100a, launched with the reference's grids "
+    out["what"] = ("reference kernel strings compiled with nvcc -O3 for sm_90a, launched with the reference's grids "
                    "(512 threads, 1 thread / pixel); wall clock around synchronised calls, median of %d" % args.reps)
     return out
 
@@ -131,7 +131,7 @@ def nmr(args):
     tf, tb = med(wall(fwd, args.reps)), med(wall(bwd, args.reps))
     return {"batch": B, "faces": nf2, "image_size": H, "texture_size": ts_, "fwd_ms": tf, "bwd_ms": tb, "step_ms": tf + tb,
             "frames_per_s": B * 1e3 / (tf + tb),
-            "what": "reference K7+K8 / K9+K10 compiled with nvcc -O3 for sm_100a, reference launch shapes, rgb mode, "
+            "what": "reference K7+K8 / K9+K10 compiled with nvcc -O3 for sm_90a, reference launch shapes, rgb mode, "
                     "no background mix / flip (host ops); wall clock around synchronised calls, median of %d" % args.reps}
 
 

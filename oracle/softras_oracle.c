@@ -40,8 +40,8 @@
  *     treating it as v0 = 0 (never hit by any test mesh; flagged in DESIGN.md).
  *
  * Parity status: pinned against outputs of the reference's own kernel strings
- * compiled for sm_100a and run on a B200 (tests/golden/ref_gpu_*.npz, generated
- * by oracle/make_ref_golden.py).  See DESIGN.md "Oracle".
+ * compiled by oracle/build_ref.py and run on a GPU (tests/golden/ref_gpu_*.npz, generated
+ * by oracle/make_ref_golden.py; each file's provenance names the GPU and nvcc flags).  See DESIGN.md "Oracle".
  */
 #include <math.h>
 #include <stdint.h>

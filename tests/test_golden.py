@@ -1,11 +1,13 @@
 """Pins the CPU oracle to the REAL reference: tests/golden/ref_gpu_*.npz hold outputs of the
 reference's own kernel strings (jrender/renderer/dr/softras/cuda/soft_rasterize.py), compiled
-for sm_100a by oracle/build_ref.py and run on a B200 by oracle/make_ref_golden.py.
+by oracle/build_ref.py and run on a GPU by oracle/make_ref_golden.py.  Each file records the GPU and
+nvcc flags it was made with in its `provenance` entry: the stored fixtures were made with an sm_100a
+build on a B200; regenerated ones (the recipe now builds for sm_90a) record an H100.
 
 The reference build contracts a*b+c into FMAs where nvcc chooses (nvcc defaults), the oracle
 and the product never do, and depth enters the colour softmax as exp((z-max)/1e-4): a 1-ulp
 difference in z moves a softmax weight by ~6e-4.  Tolerances are therefore statistical
-(measured values in profiles/parity_r01.md; thresholds ~4x above them):
+(thresholds ~4x above the measured values):
   * top-K id sets equal on >= 99.8 % of pixels (100 % on all fixtures but the sub-pixel mesh);
   * soft_colors: max |diff| <= 2e-3 (sub-pixel-triangle fixture: <= 2 % of pixels above 2e-3);
   * gradients: sum|diff| / sum|ref| <= 2e-3 (sub-pixel fixture: 5e-2);
@@ -34,7 +36,7 @@ def rel_l1(ref, got):
 def test_golden_files_present():
     assert len(FILES) >= 8
     prov = json.loads(str(np.load(FILES[0])["provenance"]))
-    assert "B200" in prov["gpu"] and "soft_rasterize.py" in prov["source"]
+    assert any(g in prov["gpu"] for g in ("B200", "H100")) and "soft_rasterize.py" in prov["source"]
 
 
 @pytest.mark.parametrize("path", FILES, ids=[os.path.basename(p)[8:-4] for p in FILES])
@@ -71,16 +73,16 @@ def test_oracle_matches_reference_kernels(path):
 
 # --------------------------------------------------------------------------- NMR (dr_type='n3mr')
 # tests/golden/ref_gpu_nmr_*.npz: outputs of the reference's K7-K11 kernel strings
-# (jrender/renderer/dr/n3mr/cuda/rasterize.py) compiled by oracle/build_ref.py and run on a B200
-# through oracle/ref_gpu.nmr_run (host semantics of n3mr.py:29-123).  Measured differences
-# (gpurun_out/golden/report_nmr.json, FMA contraction in the reference build only): face_index_map
+# (jrender/renderer/dr/n3mr/cuda/rasterize.py) compiled by oracle/build_ref.py and run on a GPU (the
+# `provenance` entry names it) through oracle/ref_gpu.nmr_run (host semantics of n3mr.py:29-123).  Measured
+# differences (the report oracle/make_ref_golden.py writes; FMA contraction in the reference build only): face_index_map
 # identical on every pixel of every fixture; weight / rgb / sampling weights <= 5e-5 (9e-4 on the
 # sub-pixel mesh), depth <= 3e-5, face_inv <= 9e-4 of values up to 146, grad_faces <= 2.6e-4 of max,
 # grad_textures <= 5e-5.  Thresholds are ~4x those.
 def test_nmr_golden_files_present():
     assert len(NMR_FILES) >= 4
     prov = json.loads(str(np.load(NMR_FILES[0])["provenance"]))
-    assert "B200" in prov["gpu"] and "n3mr/cuda/rasterize.py" in prov["source"]
+    assert any(g in prov["gpu"] for g in ("B200", "H100")) and "n3mr/cuda/rasterize.py" in prov["source"]
 
 
 @pytest.mark.parametrize("path", NMR_FILES, ids=[os.path.basename(p)[12:-4] for p in NMR_FILES])
@@ -111,7 +113,7 @@ def test_nmr_oracle_matches_reference_kernels(path):
 
 def test_bake_oracle_matches_reference_kernel_golden():
     """oracle/bake.py against the reference's own load_textures_cuda_kernel (io/utils/load_textures.py:3-101) compiled by
-    oracle/build_ref.py and run on a B200 (oracle/make_ref_golden.py --bake-only).  The reference build contracts a*b+c."""
+    oracle/build_ref.py and run on a GPU (oracle/make_ref_golden.py --bake-only).  The reference build contracts a*b+c."""
     from oracle import bake as obake
     g = np.load(os.path.join(ROOT, "tests", "golden", "ref_gpu_bake_random40_R5.npz"))
     out = obake.bake_textures_for_softras(g["image"], g["faces_uv"], g["textures_in"], g["is_update"])
@@ -121,7 +123,7 @@ def test_bake_oracle_matches_reference_kernel_golden():
 
 def test_n3mr_bake_oracle_matches_reference_kernel_golden():
     """oracle/bake.py:bake_textures_for_n3mr against the reference's own kernel (io/utils/load_textures.py:103-246, one build
-    per wrapping mode / sampling flavour, oracle/build_ref.py) run on a B200 (oracle/make_ref_golden.py --bake-only).
+    per wrapping mode / sampling flavour, oracle/build_ref.py) run on a GPU (oracle/make_ref_golden.py --bake-only).
     Bilinear: 1e-5 (the reference build contracts a*b+c).  Nearest: the same texel except where the sample point lies
     within that rounding of a texel boundary (<= 0.2 % of the texels)."""
     import glob

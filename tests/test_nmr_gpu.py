@@ -6,6 +6,8 @@ barycentric weights, depth, sampled colour, sampling indices/weights, face_inv, 
 Backward: gradients are sums over pixels accumulated in a different order (warp-parallel scans,
 float atomics) than the oracle's sequential double accumulation: max|diff| <= 2e-5 * max|oracle|.
 """
+import os
+
 import numpy as np
 import pytest
 
@@ -102,29 +104,28 @@ def test_39k_faces_forward_and_backward_properties_1024(cuda_device):
 
 
 def test_c4_against_reference_kernels_on_gpu(cuda_device):
-    """Product vs the reference's OWN K7-K11 (oracle/_ref, built from /root/reference by oracle/build_ref.py) on this
-    GPU at BASELINE config C4's size (1024^2, 2 x 39 200 faces, ts=2).  Tolerances as in tests/test_golden.py's NMR
-    fixtures: the reference build contracts a*b+c into FMAs, and its lock-protected z-test is race-dependent on exact
-    depth ties, so a handful of pixels on shared edges may go to the neighbouring face."""
-    from oracle import ref_gpu
-    if not ref_gpu.available():
-        pytest.skip("oracle/_ref/libjrender_ref.so not built (needs /root/reference at build time)")
-    faces, tex = nmr_scene(39200, batch=1, ts=2)
-    g = np.random.default_rng(0).uniform(-1, 1, (1, 1024, 1024, 3)).astype(np.float32)
-    ga = np.random.default_rng(1).uniform(-1, 1, (1, 1024, 1024)).astype(np.float32)
-    ref = ref_gpu.nmr_run(faces, tex, 1024, 0.1, 100.0, 1e-3, (0, 0, 0), (True, True, False), grads=(g, ga, None))
-    got = run_nmr_cuda(faces, tex, 1024, flags=(True, True, False), grads=(g, ga, None))
-    same = (ref["face_index_map"] == got["face_index_map"])
+    """Product vs the reference's OWN K7-K11 at BASELINE config C4's size (1024^2, 2 x 39 200 faces, ts=2).  The
+    reference side is tests/golden/parity_nmr_39200_1024.npz: the reference kernels (oracle/build_ref.py) run
+    on the GPU by oracle/make_ref_parity_golden.py, sampled at 2048 seeded pixels and the gradients of 2048 seeded
+    faces.  Tolerances as in tests/test_golden.py's NMR fixtures: the reference build contracts a*b+c into FMAs, and
+    its lock-protected z-test is race-dependent on exact depth ties, so a handful of pixels on shared edges may go to
+    the neighbouring face."""
+    from oracle import make_ref_parity_golden as mk
+    z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "parity_nmr_39200_1024.npz"))
+    faces, tex, g, ga = mk.nmr_inputs()
+    assert np.allclose(mk.checksums(faces, tex, g, ga), z["input_sums"], rtol=1e-12, atol=0), "seeded scene changed"
+    got = mk.nmr_sample(run_nmr_cuda(faces, tex, 1024, flags=(True, True, False), grads=(g, ga, None)), z["pixels"], z["faces"])
+    same = (z["face_index_map"] == got["face_index_map"])
     assert same.mean() >= 0.999, same.mean()
     # sliver faces at the sphere's poles have barycentric weights that cancel almost completely: the reference build's FMA
     # contraction moves their interpolated depth by up to ~1e-3 on a handful of pixels (measured max 1.1e-3), everything
     # else agrees to 1e-4
-    dd = np.abs(ref["depth_map"] - got["depth_map"])[same]
+    dd = np.abs(z["depth_map"] - got["depth_map"])[same]
     assert (dd > 1e-4).mean() <= 1e-3 and dd.max() <= 1e-2, ((dd > 1e-4).mean(), dd.max())
-    dc = np.abs(ref["rgb_map"] - got["rgb_map"])[same]
+    dc = np.abs(z["rgb_map"] - got["rgb_map"])[same]
     assert (dc > 2e-3).mean() <= 1e-3 and dc.max() <= 0.1, ((dc > 2e-3).mean(), dc.max())
     for k, tol in (("grad_faces", 0.05), ("grad_textures", 0.01)):
-        a, b = ref[k], got[k]
+        a, b = z[k].astype(np.float64), got[k].astype(np.float64)
         m = np.isfinite(a) & np.isfinite(b)
         assert np.abs(a[m] - b[m]).sum() / np.abs(a[m]).sum() <= tol, (k, np.abs(a[m] - b[m]).sum() / np.abs(a[m]).sum())
 

@@ -12,7 +12,7 @@ def run_oracle(fv, tex, params, grad=None, rows=None):
 
 
 def run_cuda(fv, tex, params, grad=None, device="cuda:0", want_faces_info=True):
-    """Through the public torch API -> ctypes -> C ABI -> sm_100a kernels."""
+    """Through the public torch API -> ctypes -> C ABI -> sm_90a kernels."""
     import torch
     from jrender_b200 import SoftRasterizeFunction
     dev = torch.device(device)
