@@ -6,10 +6,10 @@
 // warp sitting on a mesh pole (10x the work of its neighbours) stalls nobody.  (16x16 and 16x4 multi-warp CTAs were the
 // first two versions; stall_barrier was their top stall reason.)  Per block the warp walks its coarse bin's face list
 // (ascending face id), keeps the faces whose check_border rectangle touches the block (ordered ballot compaction), stages
-// their 160-byte records in shared memory 16 at a time, every lane marks the staged faces that cover ITS pixel in a
-// private 16-bit mask, and the lanes then walk their masks in lock-step (lowest bit = lowest face id): each pixel visits
-// its faces in ascending id exactly like the reference's `for (fn = 0; fn < nf; fn++)` (:311), minus the faces
-// check_border would skip.
+// their 160-byte records in shared memory 24 at a time (one bulk copy per record), every lane marks the staged faces that
+// cover ITS pixel in a private 24-bit mask, and the lanes then walk their masks in lock-step (lowest bit = lowest face
+// id): each pixel visits its faces in ascending id exactly like the reference's `for (fn = 0; fn < nf; fn++)` (:311),
+// minus the faces check_border would skip.
 //
 // Scheduling: `tile_counter == nullptr` -> one CTA per block (blockIdx); otherwise a persistent grid pulls blocks from an
 // atomic queue ordered by descending cost (number of (pixel, face) pairs per block, computed by k_coarse_bin and
@@ -30,12 +30,14 @@ struct __align__(16) FaceRecS {
 };
 
 #ifndef B200R_FWD_TMA
-#define B200R_FWD_TMA 0       // 1: records staged by cp.async.bulk (TMA) + mbarrier instead of LDG -> registers -> STS
+#define B200R_FWD_TMA 1       // records staged by cp.async.bulk (TMA) + mbarrier; 0: LDG -> registers -> STS.  H100, C3
+                              // (24-record rounds): forward 0.995 ms with bulk copies, 1.063 ms without
 #endif
 #ifndef B200R_FWD_MINB1
 #define B200R_FWD_MINB1 20    // resident one-warp CTAs per SM the register allocation must allow (96 registers).  H100, C3:
-                              // forward 1.08 ms at 20, 1.10 at 16, 1.29 at 24.  Spills (ptxas, sm_90a): the C3 instantiation
-                              // <2,1,false> 144 B stored / 272 B loaded at 96 registers (304 / 584 B at 80); the others 0-112 B
+                              // forward 1.08 ms at 20, 1.10 at 16, 1.29 at 24 (16-record rounds, LDG staging); with bulk
+                              // copies 1.017 at 20, 1.016 at 22, 1.017 at 18.  Spills (ptxas, sm_90a): the C3 instantiation
+                              // <2,1,false> 72 B stored / 80 B loaded at 96 registers; the others 0-52 B
 #endif
 
 // ---- mbarrier / bulk-copy (TMA) helpers ------------------------------------------------------------------------
@@ -65,7 +67,13 @@ __device__ __forceinline__ void f2_mbar_wait(unsigned long long* bar, uint32_t p
 // async-proxy writes of the next bulk copies
 __device__ __forceinline__ void f2_fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-constexpr int kFwdChunk = 16;   // records resident per warp: 16 rather than 32 keeps 24 warps resident per SM
+#ifndef B200R_FWD_CHUNK
+#define B200R_FWD_CHUNK 24    // records staged per round (a multiple of 4, <= 32).  H100, C3, bulk-copy staging: forward
+                              // 1.017 ms at 16, 0.995 at 24, 1.011 at 32 (32 costs resident CTAs: 20 no longer fit
+                              // the shared memory at K = 16)
+#endif
+constexpr int kFwdChunk = B200R_FWD_CHUNK;   // records resident per warp
+static_assert(kFwdChunk % 4 == 0 && kFwdChunk <= 32, "lane masks are 32-bit words read four at a time");
 constexpr int kFwdUnr = 4;      // coarse entries filtered per lane per pass
 
 struct FwdSmem {
@@ -518,8 +526,8 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
                 __syncwarp();
 #endif
                 // ---- per-lane face masks by transposition: lane j turns record j's rectangle, clipped to the 8x4
-                // block, into the 32-bit set of covered lanes; every lane then picks its own bit out of the 16 words
-                // (4 broadcast LDS.128).
+                // block, into the 32-bit set of covered lanes; every lane then picks its own bit out of the kFwdChunk
+                // words (kFwdChunk / 4 broadcast LDS.128).
                 uint32_t lm = 0u;
                 if (lane < m) lm = rect_lane_mask(S.rec[lane].r.rect_x, S.rec[lane].r.rect_r, tx0, tr0);
                 if (lane < CHUNK) S.lmask[lane] = lm;
