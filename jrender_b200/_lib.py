@@ -28,7 +28,7 @@ def lib():
     global _lib
     if _lib is not None:
         return _lib
-    path = os.environ.get("B200R_LIB") or _build.LIB  # B200R_LIB: development A/B builds (build.py --variant)
+    path = _build.LIB
     if not os.path.exists(path):
         raise B200RasterError(
             "libb200raster.so not built (%s). Run `python -m jrender_b200.build` "

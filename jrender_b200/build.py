@@ -44,30 +44,6 @@ def stale():
     return any(os.path.getmtime(f) > t for f in _deps() + [os.path.abspath(__file__)])
 
 
-def build_variant(name, defines, verbose=False):
-    """Development A/B aid: lib/libb200raster_<name>.so compiled with extra -D flags (selected at
-    run time with B200R_LIB=<path>).  The product library is always libb200raster.so."""
-    from concurrent.futures import ThreadPoolExecutor
-    objdir = os.path.join(OBJDIR, name)
-    os.makedirs(objdir, exist_ok=True)
-    out = os.path.join(LIBDIR, "libb200raster_%s.so" % name)
-
-    def one(src):
-        obj = os.path.join(objdir, src[:-3] + ".o")
-        cmd = [_nvcc()] + NVCC_FLAGS + ["-D" + d for d in defines] + (["-Xptxas", "-v"] if verbose else []) + \
-              ["-c", "-o", obj, os.path.join(CSRC, src)]
-        r = subprocess.run(cmd, capture_output=True, text=True)
-        if r.returncode != 0:
-            raise RuntimeError("nvcc failed for %s:\n%s" % (src, r.stderr))
-        if verbose:
-            print(r.stderr)
-        return obj
-    with ThreadPoolExecutor(max_workers=8) as ex:
-        objs = list(ex.map(one, SOURCES))
-    subprocess.run([_nvcc(), "-shared", "-o", out] + objs, check=True)
-    return out
-
-
 def build(force=False, verbose=False):
     """Compile every translation unit to an object file (in parallel), then link the .so."""
     if not force and not stale():
@@ -99,8 +75,4 @@ def build(force=False, verbose=False):
 
 
 if __name__ == "__main__":
-    if "--variant" in sys.argv:  # python -m jrender_b200.build --variant NAME -DX=1 -DY=2
-        k = sys.argv.index("--variant")
-        print(build_variant(sys.argv[k + 1], [a[2:] for a in sys.argv if a.startswith("-D")], verbose="--verbose" in sys.argv))
-    else:
-        print(build(force="--force" in sys.argv, verbose="--verbose" in sys.argv))
+    print(build(force="--force" in sys.argv, verbose="--verbose" in sys.argv))

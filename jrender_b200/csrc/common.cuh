@@ -13,6 +13,8 @@
 
 #define B200R_TILE 16          // fine tile edge in pixels (one CTA of 256 threads)
 #define B200R_TILE_THREADS 256
+#define B200R_BLOCK_W 8        // SoftRas forward block: 8x4 pixels, one warp, lane = row-major pixel index
+#define B200R_BLOCK_H 4
 #define B200R_MAX_COARSE_SIDE 16
 #define B200R_LIST_CHUNK 512            // ids per chunk of the pooled coarse lists (a multiple of the forward's 128-entry filter pass)
 #define B200R_LIST_CHUNK_SHIFT 9
@@ -45,8 +47,7 @@ struct SoftRasParams {
     float near_, far_, eps, sigma, gamma, dist_eps;  // dist_eps = ln(1/dist_eps - 1)
     int dist_func, rgb_func, alpha_func, tex_type, double_side;
     int ntx;        // 16x16 tiles per image side (backward / NMR mapping)
-    int ftw, fth;   // forward tile size in pixels (8*WX x 4*WY, WX*WY warps per CTA)
-    int fntx, fnty; // forward tiles per image row / column
+    int fntx, fnty; // forward blocks (B200R_BLOCK_W x B200R_BLOCK_H) per image row / column
     int coarse_px;  // coarse bin edge in pixels (multiple of B200R_TILE)
     int ncs;        // coarse bins per image side
     int queue_len;    // persistent scheduler: entries of tile_order (one per forward block)
@@ -69,7 +70,7 @@ struct SoftRasWorkspace {
     int* coarse_pool;    // [pool_chunks][B200R_LIST_CHUNK] face ids, ascending within a list
     int chunks_per_bin, pool_chunks;
     int* counters;       // [256] scheduler state, zeroed per launch: [0] queue head, [1] pool cursor, [64..127] cost histogram, [128..191] scatter cursors
-    int* tile_cost;      // [B*max_tiles] (pixel, face) pairs per forward tile (smallest tile 8x4)
+    int* tile_cost;      // [B*max_tiles] (pixel, face) pairs per forward block
     uint2* tile_order;   // [B*max_tiles] forward blocks, most expensive first: x = column | row << 16, y = image | (no face touches it) << 31
     size_t bytes;        // of the workspace block
 };
@@ -121,7 +122,8 @@ static inline SoftRasWorkspace b200r_carve(void* state, void* base, int B, int n
     off += b200r_align256((size_t)w.pool_chunks * B200R_LIST_CHUNK * sizeof(int));
     w.counters = (int*)(p + off);
     off += b200r_align256(256 * sizeof(int));
-    const size_t max_tiles = (size_t)ntx * ntx * 8;  // queue slots: 8 forward tiles (8x4) per 16x16 cost tile
+    // queue slots: the forward blocks of ntx x ntx 16x16 tiles
+    const size_t max_tiles = (size_t)ntx * ntx * (B200R_TILE / B200R_BLOCK_W) * (B200R_TILE / B200R_BLOCK_H);
     w.tile_cost = (int*)(p + off);
     off += b200r_align256((size_t)B * max_tiles * sizeof(int));
     w.tile_order = (uint2*)(p + off);

@@ -515,12 +515,11 @@ __device__ __forceinline__ K9Pass k9_pass(int pass, const float px[3], const flo
 // visits the samples one by one (parameters broadcast by shuffle) only for the two line scans of k9_scan, where all 32
 // lanes have pixels to work on.  d1_cross / d0_cross2 -- which pick pixels through floor / ceil -- keep the reference's
 // exact, unfused arithmetic; the per-sample quotients that only scale `dist` use the approximate reciprocal.
-#ifndef B200R_K9_MINB
-#define B200R_K9_MINB 3   // resident 256-thread CTAs per SM (80 registers, no spills).  H100, C4: 4.51 ms at 3,
-                          // 4.70 at 2 (128 registers), 4.55 at 4 (64, spills), 5.14 at 5, 5.55 at 6, 6.23 at 8 -- the scans are latency-bound
-#endif
+// resident 256-thread CTAs per SM (80 registers, no spills).  H100, C4: 4.51 ms at 3, 4.70 at 2 (128 registers), 4.55 at
+// 4 (64, spills), 5.14 at 5, 5.55 at 6, 6.23 at 8 -- the scans are latency-bound
+constexpr int kK9MinBlocks = 3;
 template <int MODE>
-__global__ void __launch_bounds__(256, B200R_K9_MINB)
+__global__ void __launch_bounds__(256, kK9MinBlocks)
 k_nmr_backward_pixel_map(const float* __restrict__ faces, const int* __restrict__ face_index_map,
                          const float* __restrict__ rgb_map, const float* __restrict__ alpha_map,
                          const float* __restrict__ ph, const float* __restrict__ pv,

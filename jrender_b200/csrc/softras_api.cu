@@ -44,12 +44,10 @@ SoftRasParams make_params(int B, int nf, int T, int is, int K, float near_, floa
     P.near_ = near_; P.far_ = far_; P.eps = eps; P.sigma = sigma; P.gamma = gamma; P.dist_eps = dist_eps;
     P.dist_func = dist; P.rgb_func = rgb; P.alpha_func = alpha; P.tex_type = tex; P.double_side = double_side ? 1 : 0;
     b200r_geometry(is, &P.ntx, &P.coarse_px, &P.ncs);
-    P.ftw = 8;   // forward blocks: one warp on 8x4 pixels
-    P.fth = 4;
     P.aa = 0;
-    P.fntx = (is + P.ftw - 1) / P.ftw;
-    P.fnty = (is + P.fth - 1) / P.fth;
-    P.queue_len = P.fntx * P.fnty * B;  // cost tiles == forward tiles: no holes
+    P.fntx = (is + B200R_BLOCK_W - 1) / B200R_BLOCK_W;
+    P.fnty = (is + B200R_BLOCK_H - 1) / B200R_BLOCK_H;
+    P.queue_len = P.fntx * P.fnty * B;  // one entry per forward block
     return P;
 }
 
@@ -115,16 +113,15 @@ static int softras_forward_impl(const float* face_vertices, const float* texture
         k_chunk_rects<<<dim3((nf + 255) / 256, B), 256, 0, st>>>(W.rects, W.chunk_rects, nf);
         k_coarse_bin<<<dim3(P.ncs * P.ncs, B), 256, 0, st>>>(W.rects, W.chunk_rects, W.coarse_cnt, W.chunk_table, W.coarse_pool, W.counters + 1,
                                                              W.chunks_per_bin, W.pool_chunks, W.tile_cost, W.counters + 64,
-                                                             nf, is, P.coarse_px, P.ncs, P.ftw, P.fth, P.fntx, P.fnty);
+                                                             nf, is, P.coarse_px, P.ncs, P.fntx, P.fnty);
     }
     e = cudaGetLastError();
     if (e != cudaSuccess) return b200r_cuda_fail(e, "k_coarse_bin");
-    // cost tiles == forward tiles: k_tile_order writes a permutation of all queue_len slots, no holes to pre-fill
+    // k_tile_order writes a permutation of all queue_len slots: no holes to pre-fill
     {
-        const int total_tiles = P.fntx * P.fnty * B;
         B200rProfScope prof(B200R_K_TILE_ORDER, st);
-        k_tile_order<<<(total_tiles + 255) / 256, 256, 0, st>>>(W.tile_cost, W.counters + 64, W.counters + 128, W.tile_order,
-                                                                B, P.fntx, P.fnty, P.ftw, P.fth, P.ftw, P.fth, P.fntx, P.fnty, 1);
+        k_tile_order<<<(P.queue_len + 255) / 256, 256, 0, st>>>(W.tile_cost, W.counters + 64, W.counters + 128, W.tile_order,
+                                                                B, P.fntx, P.fnty);
     }
     e = cudaGetLastError();
     if (e != cudaSuccess) return b200r_cuda_fail(e, "k_tile_order");

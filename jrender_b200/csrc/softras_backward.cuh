@@ -1,50 +1,30 @@
 // softras_backward.cuh -- SoftRas top-K backward (replaces K6 of the reference:
 // backward_soft_rasterize_cuda_kernel, cuda/soft_rasterize.py:1177-1360).
 //
-// The reference issues 9 + 3T scalar global atomicAdd per (pixel, face) pair.  Two variants:
+// The reference issues 9 + 3T scalar global atomicAdd per (pixel, face) pair.  Here every lane walks its own <=K saved
+// ids, reads the face record straight from the L1-resident record array, and adds its 12 gradient values (9 vertex +
+// 3 colour for T == 1) with THREE 16-byte REDG.E.ADD.F32x4 into a padded accumulator [B*nf][12];
+// k_softras_bwd_finalize then unpacks it into grad_face_vertices [.,9] and grad_textures [.,1,3] (36-byte rows cannot
+// take 16-byte atomics directly).  Atomic packets drop 4x against the reference and no zero-fill of the outputs is
+// needed.  Before the atomics of a step, lanes ^1 and ^8 (horizontal / vertical neighbour pixels) that hold the same
+// face add their values by shuffle into the lower lane (merge_same_face).
 //
-//  VARIANT 1 (default) "per-lane + vector atomics": every lane walks its own <=K saved ids, so
-//    all lanes of a covered warp work (the union walk below keeps ~48 % of the lanes busy), reads
-//    the face record straight from the L1-resident record array, and adds its 12 gradient
-//    values (9 vertex + 3 colour for T == 1) with THREE 16-byte REDG.E.ADD.F32x4 into a padded
-//    accumulator [B*nf][12]; k_softras_bwd_finalize then unpacks it into grad_face_vertices
-//    [.,9] and grad_textures [.,1,3] (36-byte rows cannot take 16-byte atomics directly).
-//    Atomic packets drop 4x against the reference and no zero-fill of the outputs is needed.
-//    (A walk in ascending face id -- ids staged and sorted in shared memory so that neighbouring lanes sit on the
-//    same record at the same step -- was measured and dropped: slower at C3; the sort costs more than the L1
-//    sectors it saves.)
-//  VARIANT 0 "warp union walk": every lane sorts its ids ascending and the warp walks the UNION
-//    of its lanes' ids (redux.sync min picks the next face); holders compute, a shuffle tree
-//    sums the 12 values and one lane issues scalar atomics: one set per (warp, face).
+// Measured and dropped, all slower at C3: a walk in ascending face id (ids staged and sorted in shared memory so that
+// neighbouring lanes sit on the same record at the same step -- the sort costs more than the L1 sectors it saves);
+// merging lanes ^2 and ^16 as well; a complete per-face reduction (match.any groups + block-floating-point REDUX.SUM,
+// several times the time of the two-level merge); a warp walking the union of its lanes' ids.
 //
-// Both evaluate the same per-pair arithmetic (pair_gradient) in the reference's order; only
-// the floating-point summation order of the atomics differs (as it does run to run in the
-// reference).
+// The per-pair arithmetic (pair_gradient) is the reference's, in its order; only the floating-point summation order of
+// the atomics differs (as it does run to run in the reference).
 #pragma once
 #include "softras_math.cuh"
 
-#ifndef B200R_BWD_MERGE
-#define B200R_BWD_MERGE 1        // warp-side aggregation levels before the atomics: 0 off, 1 = lanes ^1 and ^8, 2 = also ^2 and ^16
-                                 // (a complete per-face reduction -- match.any groups + block-floating-point REDUX.SUM --
-                                 // was measured at several times the time of level 1 at C3)
-#endif
-#ifndef B200R_BWD_MINB
+namespace b200r {
+
 // resident 256-thread CTAs per SM the backward's register allocation must allow.  Measured on the H100 at C3: 2 -> 0.675 ms,
 // 3 -> 0.606 ms, 4 -> 0.638 ms -- past 24 warps/SM the divergent 160-byte record gathers and the float atomics bind, not
 // latency.
-#define B200R_BWD_MINB 3
-#endif
-#ifndef B200R_BWD_OPTIMISTIC
-#define B200R_BWD_OPTIMISTIC 1   // 0: guarded (branching) divisions in the relaxed backward, for A/B builds
-#endif
-
-namespace b200r {
-
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) v += __shfl_xor_sync(0xffffffffu, v, d);
-    return v;
-}
+constexpr int kBwdMinBlocks = 3;
 
 // Per-pixel constants of the backward.
 struct BwdPixel {
@@ -245,7 +225,7 @@ __device__ __forceinline__ void merge_same_face(int& key, float gv[9], float gt[
 
 // ---------------------------------------------------------------- per-lane walk + vector atomics
 template <int DIST, int RGB, bool EXACT>
-__global__ void __launch_bounds__(B200R_TILE_THREADS, B200R_BWD_MINB)
+__global__ void __launch_bounds__(B200R_TILE_THREADS, kBwdMinBlocks)
 k_softras_backward_lane(const SoftRasParams P, const FaceRec* __restrict__ recs, const float* __restrict__ textures,
                         const float* __restrict__ soft_colors, const float* __restrict__ aggrs_info,
                         const int* __restrict__ ids_in, const float* __restrict__ grad_soft_colors,
@@ -261,14 +241,9 @@ k_softras_backward_lane(const SoftRasParams P, const FaceRec* __restrict__ recs,
     const size_t pn = (size_t)row * is + pxi;
     const int* src = ids_in + (size_t)b * K * npix + pn;
     int fn = valid ? __ldg(src) : -1;
-    // MERGE: the warp stays convergent (lanes whose list is empty or exhausted idle with key -1) so that lanes holding
-    // the same face can combine their contributions by shuffle before the atomics
-    constexpr bool MERGE = B200R_BWD_MERGE != 0;
-    if (MERGE) {
-        if (__all_sync(0xffffffffu, fn < 0)) return;
-    } else {
-        if (fn < 0) return;  // list ends at the first -1 (:1236)
-    }
+    // the warp stays convergent (lanes whose list is empty or exhausted idle with key -1) so that lanes holding the same
+    // face can combine their contributions by shuffle before the atomics; a list ends at the first -1 (:1236)
+    if (__all_sync(0xffffffffu, fn < 0)) return;
     const bool has_list = fn >= 0;
 
     DivConst dc;
@@ -290,14 +265,10 @@ k_softras_backward_lane(const SoftRasParams P, const FaceRec* __restrict__ recs,
     // ids are fetched two slots ahead, so the id of the NEXT face is already in a register when
     // its record is prefetched (waiting for a just-issued id load here stalled every iteration).
     // Prefetching two pairs ahead (ids three ahead) was measured too: no gain at C3.
-    const bool merge_ok = MERGE && (tex_in_acc || RGB == 2);   // texel-indexed texture gradients are not merged
+    const bool merge_ok = tex_in_acc || RGB == 2;   // texel-indexed texture gradients are not merged
     int fn_next = (1 < K && has_list) ? __ldg(src + npix) : -1;
     for (int m = 0; m < K; m++) {
-        if (MERGE) {
-            if (__all_sync(0xffffffffu, fn < 0)) break;
-        } else if (fn < 0) {
-            break;
-        }
+        if (__all_sync(0xffffffffu, fn < 0)) break;
         const int fn_next2 = (m + 2 < K && has_list) ? __ldg(src + (size_t)(m + 2) * npix) : -1;
         if (fn_next >= 0) {  // pull the next face's record (two 128-byte lines) towards L1 behind this pair's math
             const char* nr = reinterpret_cast<const char*>(brecs + fn_next);
@@ -310,10 +281,9 @@ k_softras_backward_lane(const SoftRasParams P, const FaceRec* __restrict__ recs,
         int texel;
         DivGuard guard;
         guard.ok = consts_ok;   // launch-constant denominators (sigma, gamma, far - near) validated once per thread
-        if (MERGE && fn < 0) {
+        if (fn < 0) {
             texel = 0;   // idle lane: contributes nothing, only takes part in the shuffles below
-        } else
-        if constexpr (!EXACT && B200R_BWD_OPTIMISTIC) {
+        } else if constexpr (!EXACT) {
             // all divisions branch-free; one range flag for the whole pair, one (cold) re-run if it dropped
             pair_gradient<DIST, RGB, false, true>(rec, fn, px, P, dc, nmf, r_nmf, s_nmf, btex + (size_t)fn * T * 3, gv, gt, texel, guard);
             if (!guard.ok) {
@@ -331,10 +301,6 @@ k_softras_backward_lane(const SoftRasParams P, const FaceRec* __restrict__ recs,
             // (~250 G adds/s measured at C2, C3 and C5 alike), so every merged pair of lanes is time saved
             merge_same_face<1, RGB>(key, gv, gt, lane);   // horizontal neighbour
             merge_same_face<8, RGB>(key, gv, gt, lane);   // vertical neighbour
-#if B200R_BWD_MERGE >= 2
-            merge_same_face<2, RGB>(key, gv, gt, lane);
-            merge_same_face<16, RGB>(key, gv, gt, lane);
-#endif
         }
         if (key >= 0) {
             float4* a = reinterpret_cast<float4*>(bacc + (size_t)key * 12);

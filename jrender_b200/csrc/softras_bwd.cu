@@ -36,7 +36,11 @@ cudaError_t b200r_launch_backward(const SoftRasParams& P, const SoftRasWorkspace
         e = cudaMemsetAsync(grad_textures, 0, sizeof(float) * 3 * (size_t)P.T * nfaces, st);
         if (e != cudaSuccess) return e;
     }
-    B200R_DISPATCH_DIST_RGB((e = (D == 2 && !exact) ? launch_lane<D, R, (D != 2)>(P, W, textures, soft_colors, aggrs_info, ids, grad_soft_colors, grad_textures, st) : launch_lane<D, R, true>(P, W, textures, soft_colors, aggrs_info, ids, grad_soft_colors, grad_textures, st)))
+    decltype(&launch_lane<2, 1, true>) launch = nullptr;
+    // fp32 tails + optimistic divisions only for the default euclidean distance, as in the forward
+    B200R_DISPATCH_DIST_RGB(if constexpr (D == 2) launch = exact ? launch_lane<D, R, true> : launch_lane<D, R, false>;
+                            else launch = launch_lane<D, R, true>)
+    e = launch(P, W, textures, soft_colors, aggrs_info, ids, grad_soft_colors, grad_textures, st);
     if (e != cudaSuccess) return e;
     {
         B200rProfScope prof(B200R_K_SOFTRAS_BWD_FINALIZE, st);

@@ -29,18 +29,16 @@ struct __align__(16) FaceRecS {
     uint4 pad;
 };
 
-#ifndef B200R_FWD_TMA
-#define B200R_FWD_TMA 1       // records staged by cp.async.bulk (TMA) + mbarrier; 0: LDG -> registers -> STS.  H100, C3
-                              // (24-record rounds): forward 0.995 ms with bulk copies, 1.063 ms without
-#endif
-#ifndef B200R_FWD_MINB1
-#define B200R_FWD_MINB1 20    // resident one-warp CTAs per SM the register allocation must allow (96 registers).  H100, C3:
-                              // forward 1.08 ms at 20, 1.10 at 16, 1.29 at 24 (16-record rounds, LDG staging); with bulk
-                              // copies 1.017 at 20, 1.016 at 22, 1.017 at 18.  Spills (ptxas, sm_90a): the C3 instantiation
-                              // <2,1,false> 72 B stored / 80 B loaded at 96 registers; the others 0-52 B
-#endif
+constexpr int kFwdLanes = 32;   // one warp per B200R_BLOCK_W x B200R_BLOCK_H block
+static_assert(B200R_BLOCK_W * B200R_BLOCK_H == kFwdLanes, "one lane per pixel of the block");
 
-// ---- mbarrier / bulk-copy (TMA) helpers ------------------------------------------------------------------------
+// resident one-warp CTAs per SM the register allocation must allow (96 registers).  H100, C3: forward 1.08 ms at 20, 1.10
+// at 16, 1.29 at 24 (16-record rounds, LDG staging); with bulk copies 1.017 at 20, 1.016 at 22, 1.017 at 18.  Spills
+// (ptxas, sm_90a): the C3 instantiation <2,1,false> 72 B stored / 80 B loaded at 96 registers; the others 0-52 B
+constexpr int kFwdMinBlocks = 20;
+
+// ---- mbarrier / bulk-copy (TMA) helpers.  Records are staged by cp.async.bulk + mbarrier rather than LDG -> registers
+// -> STS: H100, C3 (24-record rounds), forward 0.995 ms with bulk copies, 1.063 ms with LDG staging
 __device__ __forceinline__ uint32_t f2_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void f2_mbar_init(unsigned long long* bar, int count) {
     asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(f2_smem_u32(bar)), "r"(count) : "memory");
@@ -67,12 +65,9 @@ __device__ __forceinline__ void f2_mbar_wait(unsigned long long* bar, uint32_t p
 // async-proxy writes of the next bulk copies
 __device__ __forceinline__ void f2_fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-#ifndef B200R_FWD_CHUNK
-#define B200R_FWD_CHUNK 24    // records staged per round (a multiple of 4, <= 32).  H100, C3, bulk-copy staging: forward
-                              // 1.017 ms at 16, 0.995 at 24, 1.011 at 32 (32 costs resident CTAs: 20 no longer fit
-                              // the shared memory at K = 16)
-#endif
-constexpr int kFwdChunk = B200R_FWD_CHUNK;   // records resident per warp
+// records staged per round (a multiple of 4, <= 32).  H100, C3, bulk-copy staging: forward 1.017 ms at 16, 0.995 at 24,
+// 1.011 at 32 (32 costs resident CTAs: 20 no longer fit the shared memory at K = 16)
+constexpr int kFwdChunk = 24;
 static_assert(kFwdChunk % 4 == 0 && kFwdChunk <= 32, "lane masks are 32-bit words read four at a time");
 constexpr int kFwdUnr = 4;      // coarse entries filtered per lane per pass
 
@@ -80,7 +75,7 @@ struct FwdSmem {
     FaceRecS rec[kFwdChunk];                   // staged records; reused as the output staging area
     int ids[kFwdChunk + kFwdUnr * 32];         // pending block-face ids, ascending
     __align__(16) uint32_t lmask[kFwdChunk];   // per staged record, the lanes whose pixel it covers
-    unsigned long long mbar;                   // B200R_FWD_TMA: completion barrier of the bulk copies
+    unsigned long long mbar;                   // completion barrier of the bulk copies
     unsigned long long pad_;
 };
 static_assert(sizeof(FwdSmem) % 16 == 0, "the top-K depth lists behind FwdSmem are read with 16-byte loads");
@@ -102,18 +97,17 @@ struct PixState {
 };
 
 // top-K by z with the reference's "replace the current max" policy (:367-385).  my_qz = this pixel's K depths
-// (16-byte aligned, slot order), s_qid = ids [K][NT].  The rescan after a replacement is the reference's loop
+// (16-byte aligned, slot order), s_qid = ids [K][32].  The rescan after a replacement is the reference's loop
 // (first strictly greater depth wins, so ties keep the lowest slot) reading four slots per LDS.128.
-template <int NT>
 __device__ __forceinline__ void topk_insert(PixState& st, float zp, int fn, int K, float* my_qz, int* s_qid, int tid) {
     if (st.q_size < K) {
         my_qz[st.q_size] = zp;
-        s_qid[st.q_size * NT + tid] = fn;
+        s_qid[st.q_size * kFwdLanes + tid] = fn;
         if (zp > st.q_max_z) { st.q_max_z = zp; st.q_max_id = st.q_size; }
         st.q_size++;
     } else if (zp < st.q_max_z) {
         my_qz[st.q_max_id] = zp;
-        s_qid[st.q_max_id * NT + tid] = fn;
+        s_qid[st.q_max_id * kFwdLanes + tid] = fn;
         float m = -1.f;
         int id = st.q_max_id;
         int k = 0;
@@ -135,7 +129,7 @@ __device__ __forceinline__ void topk_insert(PixState& st, float zp, int fn, int 
 
 // The reference's per-face loop body (:318-420) for one (pixel, face) pair whose pixel is
 // inside the face's check_border rectangle.
-template <int DIST, int RGB, int NT, bool EXACT>
+template <int DIST, int RGB, bool EXACT>
 __device__ __forceinline__ void shade_face(const FaceRec* rec, PixState& st, const SoftRasParams& P, const DivConst& dc,
                                            float xp, float yp, float threshold, float* s_qz, int* s_qid, int tid,
                                            const float* __restrict__ btex) {
@@ -172,7 +166,7 @@ __device__ __forceinline__ void shade_face(const FaceRec* rec, PixState& st, con
     if (zp < P.near_ || zp > P.far_) return;       // :365
 
     const int fn = (int)rec->face_id;
-    topk_insert<NT>(st, zp, fn, P.K, s_qz, s_qid, tid);   // s_qz = this pixel's depth list
+    topk_insert(st, zp, fn, P.K, s_qz, s_qid, tid);   // s_qz = this pixel's depth list
 
     const bool front = (rec->flags & 8u) != 0;
     if (RGB == 0) {  // :390-397
@@ -202,17 +196,13 @@ __device__ __forceinline__ void shade_face(const FaceRec* rec, PixState& st, con
     }
 }
 
-#ifndef B200R_FWD_OPTIMISTIC
-#define B200R_FWD_OPTIMISTIC 1   // 0: shade_face with guarded (branching) divisions only, for A/B builds
-#endif
-
 // shade_face with every division in its branch-free optimistic form (exact_math.cuh, DivGuard): the pair's
 // arithmetic up to the first state update runs without a single range branch, the range conditions are AND-ed
 // into one flag, and a pair whose flag dropped (practically never) is handed to shade_face above before anything
 // was committed.  With the flag up every intermediate equals shade_face<.., EXACT = false>'s bit for bit:
 // same Markstein sequences, and the two exp() of the online softmax collapse into one because
 // exp((max - z)/gamma) and exp((z - max)/gamma) are never both different from 1.
-template <int DIST, int RGB, int NT>
+template <int DIST, int RGB>
 __device__ __forceinline__ void shade_face_opt(const FaceRec* rec, PixState& st, const SoftRasParams& P, const DivConst& dc,
                                                float xp, float yp, float threshold, float* s_qz, int* s_qid, int tid,
                                                const float* __restrict__ btex, bool consts_ok) {
@@ -245,7 +235,7 @@ __device__ __forceinline__ void shade_face_opt(const FaceRec* rec, PixState& st,
         ex = expf(dc.by_gamma_o(-fabsf(dz), g));   // = exp_delta_zp when dz > 0, exp_z otherwise (:402-407)
     }
     if (!g.ok) {  // cold: nothing has been committed yet
-        shade_face<DIST, RGB, NT, false>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, tid, btex);
+        shade_face<DIST, RGB, false>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, tid, btex);
         return;
     }
 
@@ -260,7 +250,7 @@ __device__ __forceinline__ void shade_face_opt(const FaceRec* rec, PixState& st,
     if (zp < P.near_ || zp > P.far_) return;       // :365
 
     const int fn = (int)rec->face_id;
-    topk_insert<NT>(st, zp, fn, P.K, s_qz, s_qid, tid);   // s_qz = this pixel's depth list
+    topk_insert(st, zp, fn, P.K, s_qz, s_qid, tid);   // s_qz = this pixel's depth list
 
     const bool front = (rec->flags & 8u) != 0;
     if (RGB == 0) {  // :390-397
@@ -288,12 +278,12 @@ __device__ __forceinline__ void shade_face_opt(const FaceRec* rec, PixState& st,
 }
 
 // EXACT (softras_exact_tail = 1) keeps the reference's double-precision tails and the strictly guarded divisions.
-template <int DIST, int RGB, int NT, bool EXACT>
+template <int DIST, int RGB, bool EXACT>
 __device__ __forceinline__ void shade_pair(const FaceRec* rec, PixState& st, const SoftRasParams& P, const DivConst& dc,
                                            float xp, float yp, float threshold, float* s_qz, int* s_qid, int tid,
                                            const float* __restrict__ btex, bool consts_ok) {
-    if constexpr (!EXACT && B200R_FWD_OPTIMISTIC) shade_face_opt<DIST, RGB, NT>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, tid, btex, consts_ok);
-    else shade_face<DIST, RGB, NT, EXACT>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, tid, btex);
+    if constexpr (!EXACT) shade_face_opt<DIST, RGB>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, tid, btex, consts_ok);
+    else shade_face<DIST, RGB, EXACT>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, tid, btex);
 }
 
 // Anti-aliasing epilogue (SoftRasterizer.execute renders at 2x and mean-pools 2x2, rasterizer.py:45,54-55): the 2x2 means
@@ -343,13 +333,13 @@ __device__ __forceinline__ void finalize_pixel(const PixState& st, const SoftRas
 }
 
 template <int DIST, int RGB, bool EXACT>
-__global__ void __launch_bounds__(32, B200R_FWD_MINB1)
+__global__ void __launch_bounds__(32, kFwdMinBlocks)
 k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const uint2* __restrict__ rects,
                   const int* __restrict__ coarse_cnt, const int* __restrict__ chunk_table,
                   const int* __restrict__ coarse_pool, const int chunks_per_bin, const float* __restrict__ textures, float* __restrict__ soft_colors,
                   float* __restrict__ aggrs_info, int* __restrict__ ids_out, int* tile_counter,
                   const uint2* __restrict__ tile_order, float* __restrict__ pooled) {
-    constexpr int NT = 32, CHUNK = kFwdChunk, UNR = kFwdUnr, TW = 8, TH = 4;
+    constexpr int NT = kFwdLanes, CHUNK = kFwdChunk, UNR = kFwdUnr, TW = B200R_BLOCK_W, TH = B200R_BLOCK_H;
     constexpr unsigned FULL = 0xffffffffu;
     extern __shared__ __align__(16) unsigned char smem_raw[];
     FwdSmem& S = *reinterpret_cast<FwdSmem*>(smem_raw);
@@ -369,11 +359,9 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
     const uint32_t lt_mask = (1u << lane) - 1u;
     const bool vec_out = (is & 3) == 0;
     const bool vec_ids = vec_out && ((K & 3) == 0);
-#if B200R_FWD_TMA
     if (lane == 0) f2_mbar_init(&S.mbar, 1);
     __syncwarp();
     uint32_t parity = 0;
-#endif
 
     for (int titer = 0;; titer++) {
         // ---- which block
@@ -494,7 +482,6 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
             while (n_pending >= CHUNK || (last && n_pending > 0)) {
                 const int m = min(n_pending, CHUNK);
                 __syncwarp();  // S.ids complete; previous round's readers of S.rec done
-#if B200R_FWD_TMA
                 // ---- stage m records: one 160-byte bulk copy each, completion counted in bytes on the mbarrier
                 f2_fence_async_smem();
                 if (lane == 0) f2_mbar_expect_tx(&S.mbar, (uint32_t)m * (uint32_t)sizeof(FaceRec));
@@ -502,29 +489,6 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
                 if (lane < m) f2_bulk_g2s(&S.rec[lane].r, brecs + S.ids[head + lane], (uint32_t)sizeof(FaceRec), &S.mbar);
                 f2_mbar_wait(&S.mbar, parity);
                 parity ^= 1u;
-#else
-                // ---- stage m records: 10 x uint4 per face, coalesced, 5 loads in flight per lane
-                for (int j0 = 0; j0 < m * B200R_REC_UINT4; j0 += NT * 5) {
-                    uint4 v[5];
-#pragma unroll
-                    for (int u = 0; u < 5; u++) {
-                        const int j = j0 + u * NT + lane;
-                        if (j < m * B200R_REC_UINT4) {
-                            const int f = j / B200R_REC_UINT4, q = j - f * B200R_REC_UINT4;
-                            v[u] = __ldg(reinterpret_cast<const uint4*>(brecs + S.ids[head + f]) + q);
-                        }
-                    }
-#pragma unroll
-                    for (int u = 0; u < 5; u++) {
-                        const int j = j0 + u * NT + lane;
-                        if (j < m * B200R_REC_UINT4) {
-                            const int f = j / B200R_REC_UINT4, q = j - f * B200R_REC_UINT4;
-                            reinterpret_cast<uint4*>(&S.rec[f])[q] = v[u];
-                        }
-                    }
-                }
-                __syncwarp();
-#endif
                 // ---- per-lane face masks by transposition: lane j turns record j's rectangle, clipped to the 8x4
                 // block, into the 32-bit set of covered lanes; every lane then picks its own bit out of the kFwdChunk
                 // words (kFwdChunk / 4 broadcast LDS.128).
@@ -547,7 +511,7 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
                     if (mask != 0u) {
                         const FaceRec* rec = &S.rec[__ffs(mask) - 1].r;
                         mask &= mask - 1u;
-                        shade_pair<DIST, RGB, NT, EXACT>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, lane, btex, consts_ok);
+                        shade_pair<DIST, RGB, EXACT>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, lane, btex, consts_ok);
                     }
                 }
                 head += m;

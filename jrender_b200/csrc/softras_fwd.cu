@@ -11,8 +11,8 @@ namespace {
 constexpr int MAXDEV = 64;   // function attributes and occupancy are per DEVICE: cached per ordinal
 
 template <int DIST, int RGB, bool EXACT>
-cudaError_t launch_v1(const SoftRasParams& P, const SoftRasWorkspace& W, const float* textures, float* soft_colors,
-                      float* aggrs_info, int32_t* ids, float* pooled, int persistent, cudaStream_t st) {
+cudaError_t launch_forward(const SoftRasParams& P, const SoftRasWorkspace& W, const float* textures, float* soft_colors,
+                           float* aggrs_info, int32_t* ids, float* pooled, int persistent, cudaStream_t st) {
     const size_t smem = fwd_smem_bytes(P.K);
     static std::atomic<size_t> cfg_smem[MAXDEV];
     static std::atomic<int> cfg_occ[MAXDEV];
@@ -59,8 +59,9 @@ cudaError_t launch_v1(const SoftRasParams& P, const SoftRasWorkspace& W, const f
 
 cudaError_t b200r_launch_forward(const SoftRasParams& P, const SoftRasWorkspace& W, const float* textures, float* soft_colors,
                                  float* aggrs_info, int32_t* ids, float* pooled, int persistent, int exact, cudaStream_t st) {
-    cudaError_t e = cudaSuccess;
+    decltype(&launch_forward<2, 1, true>) launch = nullptr;
     // fp32 tails + optimistic divisions only for the default euclidean distance; the other modes keep the exact tails
-    B200R_DISPATCH_DIST_RGB((e = (D == 2 && !exact) ? launch_v1<D, R, (D != 2)>(P, W, textures, soft_colors, aggrs_info, ids, pooled, persistent, st) : launch_v1<D, R, true>(P, W, textures, soft_colors, aggrs_info, ids, pooled, persistent, st)))
-    return e;
+    B200R_DISPATCH_DIST_RGB(if constexpr (D == 2) launch = exact ? launch_forward<D, R, true> : launch_forward<D, R, false>;
+                            else launch = launch_forward<D, R, true>)
+    return launch(P, W, textures, soft_colors, aggrs_info, ids, pooled, persistent, st);
 }

@@ -14,15 +14,16 @@ cudaError_t b200r_launch_backward(const SoftRasParams& P, const SoftRasWorkspace
                                   const float* grad_soft_colors, float* grad_faces, float* grad_textures,
                                   int exact, cudaStream_t st);
 
-#define B200R_DISPATCH_DIST_RGB(CALL)                               \
-    switch (P.dist_func * 3 + P.rgb_func) {                         \
-        case 0: { constexpr int D = 0, R = 0; CALL; } break;        \
-        case 1: { constexpr int D = 0, R = 1; CALL; } break;        \
-        case 2: { constexpr int D = 0, R = 2; CALL; } break;        \
-        case 3: { constexpr int D = 1, R = 0; CALL; } break;        \
-        case 4: { constexpr int D = 1, R = 1; CALL; } break;        \
-        case 5: { constexpr int D = 1, R = 2; CALL; } break;        \
-        case 6: { constexpr int D = 2, R = 0; CALL; } break;        \
-        case 7: { constexpr int D = 2, R = 1; CALL; } break;        \
-        default: { constexpr int D = 2, R = 2; CALL; } break;       \
+// runs the statement(s) with D = P.dist_func and R = P.rgb_func as compile-time constants
+#define B200R_DISPATCH_DIST_RGB(...)                                       \
+    switch (P.dist_func * 3 + P.rgb_func) {                                \
+        case 0: { constexpr int D = 0, R = 0; __VA_ARGS__; } break;        \
+        case 1: { constexpr int D = 0, R = 1; __VA_ARGS__; } break;        \
+        case 2: { constexpr int D = 0, R = 2; __VA_ARGS__; } break;        \
+        case 3: { constexpr int D = 1, R = 0; __VA_ARGS__; } break;        \
+        case 4: { constexpr int D = 1, R = 1; __VA_ARGS__; } break;        \
+        case 5: { constexpr int D = 1, R = 2; __VA_ARGS__; } break;        \
+        case 6: { constexpr int D = 2, R = 0; __VA_ARGS__; } break;        \
+        case 7: { constexpr int D = 2, R = 1; __VA_ARGS__; } break;        \
+        default: { constexpr int D = 2, R = 2; __VA_ARGS__; } break;       \
     }

@@ -127,10 +127,9 @@ __device__ __forceinline__ bool rect_overlaps(uint2 rc, int x0, int x1, int r0, 
     return fx0 <= x1 && fx1 >= x0 && fr0 <= r1 && fr1 >= r0 && fx0 <= fx1;
 }
 
-// Block-wide ORDERED compaction step: thread `tid` contributes `cnt` items; returns the
-// exclusive prefix over the block (in thread order) and the block total.  NW warps per block.
-template <int NW>
-__device__ __forceinline__ int block_excl_scan(int cnt, int* s_warp /*[NW]*/, int& total) {
+// Block-wide ORDERED compaction step of a 256-thread (8-warp) block: thread `tid` contributes `cnt` items; returns the
+// exclusive prefix over the block (in thread order) and the block total.
+__device__ __forceinline__ int block_excl_scan(int cnt, int* s_warp /*[8]*/, int& total) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     int incl = cnt;
 #pragma unroll
@@ -138,15 +137,11 @@ __device__ __forceinline__ int block_excl_scan(int cnt, int* s_warp /*[NW]*/, in
         const int n = __shfl_up_sync(0xffffffffu, incl, d);
         if (lane >= d) incl += n;
     }
-    if (NW == 1) {
-        total = __shfl_sync(0xffffffffu, incl, 31);
-        return incl - cnt;
-    }
     if (lane == 31) s_warp[warp] = incl;
     __syncthreads();
     int base = 0, tot = 0;
 #pragma unroll
-    for (int wi = 0; wi < NW; wi++) {
+    for (int wi = 0; wi < 8; wi++) {
         const int v = s_warp[wi];
         if (wi < warp) base += v;
         tot += v;
@@ -156,20 +151,15 @@ __device__ __forceinline__ int block_excl_scan(int cnt, int* s_warp /*[NW]*/, in
     return base + incl - cnt;
 }
 // Same for a 0/1 contribution: one ballot instead of a 5-step shuffle scan.
-template <int NW>
-__device__ __forceinline__ int block_excl_scan_flag(bool flag, int* s_warp /*[NW]*/, int& total) {
+__device__ __forceinline__ int block_excl_scan_flag(bool flag, int* s_warp /*[8]*/, int& total) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const unsigned bal = __ballot_sync(0xffffffffu, flag);
     const int excl = __popc(bal & ((1u << lane) - 1u));
-    if (NW == 1) {
-        total = __popc(bal);
-        return excl;
-    }
     if (lane == 0) s_warp[warp] = __popc(bal);
     __syncthreads();
     int base = 0, tot = 0;
 #pragma unroll
-    for (int wi = 0; wi < NW; wi++) {
+    for (int wi = 0; wi < 8; wi++) {
         const int v = s_warp[wi];
         if (wi < warp) base += v;
         tot += v;
@@ -178,7 +168,6 @@ __device__ __forceinline__ int block_excl_scan_flag(bool flag, int* s_warp /*[NW
     total = tot;
     return base + excl;
 }
-__device__ __forceinline__ int block_excl_scan_256(int cnt, int* s_warp, int& total) { return block_excl_scan<8>(cnt, s_warp, total); }
 
 // Coarse binning, tile-centric and deterministic: CTA (bin, b) scans the face rectangles of
 // batch element b in ascending face id and appends the overlapping ids, in order, to its
@@ -232,10 +221,11 @@ static __global__ void __launch_bounds__(256) k_coarse_bin(const uint2* __restri
                                                     int* __restrict__ coarse_pool, int* __restrict__ pool_cursor,
                                                     int chunks_per_bin, int pool_chunks, int* __restrict__ tile_cost,
                                                     int* __restrict__ cost_hist, int nf, int is,
-                                                    int coarse_px, int ncs, int tw, int th, int ntx, int nty) {
+                                                    int coarse_px, int ncs, int ntx, int nty) {
+    constexpr int tw = B200R_BLOCK_W, th = B200R_BLOCK_H;   // cost per forward block
     __shared__ int s_warp[8];
     __shared__ int s_hist[B200R_COST_BUCKETS];
-    __shared__ int s_cost[2048];  // tiles of this bin: (coarse_px/tw) * (coarse_px/th) <= 32 * 64 (8x4 tiles, 256 px bins)
+    __shared__ int s_cost[2048];  // blocks of this bin: (coarse_px/tw) * (coarse_px/th) <= 32 * 64 (256 px bins)
     __shared__ int s_overflow;
     __shared__ int s_chunk[4];    // [0]: the chunk the list currently ends in; [1..3]: chunks allocated for the current pass
     __shared__ int s_hits[256];   // passes of the current group of 256 that touch the bin, ascending
@@ -285,7 +275,7 @@ static __global__ void __launch_bounds__(256) k_coarse_bin(const uint2* __restri
             }
         }
         int n_hit;
-        const int hpos = block_excl_scan_flag<8>(hit, s_warp, n_hit);
+        const int hpos = block_excl_scan_flag(hit, s_warp, n_hit);
         if (hit) s_hits[hpos] = my_pass;
         __syncthreads();
 
@@ -303,7 +293,7 @@ static __global__ void __launch_bounds__(256) k_coarse_bin(const uint2* __restri
             for (int u = 0; u < PT; u++)
                 if (rect_overlaps(rr[u], x0, x1, r0, r1)) mask |= 1u << u;
             int total;
-            int off = n_out + block_excl_scan_256(__popc(mask), s_warp, total);
+            int off = n_out + block_excl_scan(__popc(mask), s_warp, total);
             if (!overflow) {
                 // chunks for list positions [n_out, n_out + total): the list so far ends inside chunk number have - 1
                 const int have = (n_out + B200R_LIST_CHUNK - 1) >> B200R_LIST_CHUNK_SHIFT;
@@ -378,23 +368,21 @@ static __global__ void __launch_bounds__(256) k_coarse_bin(const uint2* __restri
     if (threadIdx.x < B200R_COST_BUCKETS && s_hist[threadIdx.x] > 0) atomicAdd(&cost_hist[threadIdx.x], s_hist[threadIdx.x]);
 }
 
-// Orders all forward tiles by descending cost bucket (longest-processing-time-first for the
-// persistent raster grid).  Costs are kept per (ctw x cth) "cost tile" (k_coarse_bin); a forward
-// tile of (tw x th) pixels inherits the bucket of the cost tile that contains it.  hist[] counts
-// COST tiles per bucket (complete after k_coarse_bin); `per` = forward tiles per cost tile (1 when
-// the two tilings coincide, which is how the SoftRas forward runs: a silhouette tile whose only
-// busy 8x4 block is long-running must not hide behind its cheap 16x16 parent).  Block-aggregated
-// reservation: one global atomic per (CTA, bucket) instead of one per tile.
+// Orders all forward blocks by descending cost bucket (longest-processing-time-first for the
+// persistent raster grid): each queue entry takes the bucket of its own block's cost (k_coarse_bin),
+// so a silhouette block that is long-running starts early even when its neighbours are cheap.
+// hist[] counts blocks per bucket (complete after k_coarse_bin).  Block-aggregated reservation:
+// one global atomic per (CTA, bucket) instead of one per block.
 static __global__ void __launch_bounds__(256) k_tile_order(const int* __restrict__ tile_cost, const int* __restrict__ hist,
                                                            int* __restrict__ cursor, uint2* __restrict__ tile_order,
-                                                           int B, int fntx, int fnty, int tw, int th, int ctw, int cth, int cntx, int cnty, int per) {
+                                                           int B, int fntx, int fnty) {
     __shared__ int s_start[B200R_COST_BUCKETS];
     __shared__ int s_cnt[B200R_COST_BUCKETS];
     __shared__ int s_base[B200R_COST_BUCKETS];
     if (threadIdx.x < B200R_COST_BUCKETS) s_cnt[threadIdx.x] = 0;
     if (threadIdx.x == 0) {
         int acc = 0;
-        for (int k = B200R_COST_BUCKETS - 1; k >= 0; k--) { s_start[k] = acc; acc += hist[k] * per; }
+        for (int k = B200R_COST_BUCKETS - 1; k >= 0; k--) { s_start[k] = acc; acc += hist[k]; }
     }
     __syncthreads();
     const int total = B * fntx * fnty;
@@ -403,9 +391,8 @@ static __global__ void __launch_bounds__(256) k_tile_order(const int* __restrict
     uint2 entry = make_uint2(0u, 0u);
     if (t < total) {
         const int b = t / (fntx * fnty), tt = t % (fntx * fnty);
-        const int cx = (tt % fntx) * tw / ctw, cy = (tt / fntx) * th / cth;
         entry.x = (uint32_t)(tt % fntx) | ((uint32_t)(tt / fntx) << 16);
-        bkt = cost_bucket(tile_cost[(size_t)b * cntx * cnty + cy * cntx + cx]);
+        bkt = cost_bucket(tile_cost[t]);   // [B][fnty][fntx], the order of t
         lrank = atomicAdd(&s_cnt[bkt], 1);
         entry.y = (uint32_t)b | (bkt == 0 ? 0x80000000u : 0u);   // bucket 0 <=> no rectangle touches the block (exact count)
     }
