@@ -6,7 +6,9 @@ squared differences to a reference image from a random azimuth) and optimiser (A
 The reference fits `data/ref/ref_texture.png`; by default this script fits a render of the cow with its own baked texture
 from a fixed azimuth, which keeps it self-contained:
 
-    python examples/demo4_optim_textures.py [--iters 200] [-ir ref.png]
+    python examples/demo4_optim_textures.py [--iters 200] [-ir ref.png] [--save out/cow.obj]
+
+`--save` writes the fitted cow through Mesh.save_obj(save_texture=True) (.obj + .mtl + texture-atlas .png).
 """
 import argparse
 import os
@@ -74,14 +76,29 @@ def run(filename_obj=DEFAULT_OBJ, filename_ref=None, iters=200, device='cuda:0',
     return model, losses
 
 
-def main():
+def save(model, filename_obj, texture_res_out=16):
+    """Write the fitted cow (the model's vertices, tanh of the texture parameter) as .obj + .mtl + .png: the NMR texture
+    volumes go through the texture-atlas export (Mesh.save_obj(save_texture=True)), so another tool can open the result
+    and Mesh.from_obj(..., load_texture=True, dr_type='n3mr') reads it back."""
+    d = os.path.dirname(os.path.abspath(filename_obj))
+    os.makedirs(d, exist_ok=True)
+    with torch.no_grad():
+        mesh = jr.Mesh(model.vertices, model.faces, torch.tanh(model.textures), dr_type='n3mr')
+    mesh.save_obj(filename_obj, save_texture=True, texture_res_out=texture_res_out)
+
+
+def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument('-io', '--filename_obj', type=str, default=DEFAULT_OBJ)
     ap.add_argument('-ir', '--filename_ref', type=str, default=None)
     ap.add_argument('--iters', type=int, default=200)
-    args = ap.parse_args()
+    ap.add_argument('--save', type=str, default=None, metavar='PATH', help='write the fitted textured mesh to PATH (.obj, + .mtl / .png)')
+    args = ap.parse_args(argv)
     model, losses = run(args.filename_obj, args.filename_ref, args.iters, log=20)
     print("loss %.3f -> %.3f" % (losses[0], losses[-1]))
+    if args.save:
+        save(model, args.save)
+        print("saved %s" % args.save)
 
 
 if __name__ == '__main__':

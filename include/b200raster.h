@@ -229,6 +229,24 @@ B200R_API int b200r_bake_textures_n3mr(const float* image, const float* faces_uv
                                        int nf, int texture_size, int image_height, int image_width, int texture_wrapping,
                                        int use_bilinear, void* stream);
 
+/* ---- texture-atlas export (the inverse of the bake) ------------------------------------------------------------
+ * Replaces create_texture_image_cuda_kernel (jrender/io/utils/create_texture_image.py:3-104), called from
+ * create_texture_image, jrender/io/save_obj.py:7-29: paints every face's texels into its texture_res_out^2 tile of
+ * image [H, W, 3] f32 (W = tile_width * texture_res_out; face fn owns tile (fn % tile_width, fn / tile_width); rows top
+ * down, the caller flips), through the face's tile triangle tile_vertices [nf, 3, 2] in pixel units.  Every pixel is
+ * written: those of tiles past the last face are set to 1.  texture_res_out must be 2 or >= 4 (at 3 the tile triangle
+ * is degenerate).  Device pointers.
+ *   softras: textures [nf, R*R, 3], R = texture_res >= 1; each pixel copies one texel (the texel index is clamped to
+ *            the face's own texels, where the reference reads unchecked).
+ *   n3mr:    textures [nf, ts, ts, ts, 3], ts = texture_size >= 2; each pixel samples the face's volume trilinearly at
+ *            its barycentric weights times (ts - 1), as the NMR forward sampler does (no reference counterpart). */
+B200R_API int b200r_texture_atlas_softras(const float* tile_vertices, const float* textures, float* image, int nf,
+                                          int texture_res, int texture_res_out, int tile_width, int image_height,
+                                          int image_width, void* stream);
+B200R_API int b200r_texture_atlas_n3mr(const float* tile_vertices, const float* textures, float* image, int nf,
+                                       int texture_size, int texture_res_out, int tile_width, int image_height,
+                                       int image_width, void* stream);
+
 /* ---- fused surface-mode lighting of the pre-raster stage (SURVEY.md section 8f rank 1) -------------------------
  * Replaces Lighting.execute with light_mode='surface', no normal map, no SSS, one directional light:
  *   jrender/renderer/lighting/lighting.py:186-204, ambient_lighting.py:4-9, directional_lighting.py:54-135
@@ -269,7 +287,7 @@ enum { B200R_K_FACE_SETUP = 0, B200R_K_COARSE_BIN = 1, B200R_K_SOFTRAS_FWD = 2, 
        B200R_K_TILE_ORDER = 4, B200R_K_NMR_SETUP = 5, B200R_K_NMR_FWD = 6, B200R_K_NMR_BWD_PIXEL = 7,
        B200R_K_NMR_BWD_MAPS = 8, B200R_K_SOFTRAS_BWD_FINALIZE = 9, B200R_K_NMR_PACK = 10,
        B200R_K_PROJECT_FWD = 11, B200R_K_PROJECT_BWD = 12, B200R_K_FLATTEN_LOSS = 13, B200R_K_LAPLACIAN_LOSS = 14,
-       B200R_K_LIGHTING = 15, B200R_K_BAKE = 16 };
+       B200R_K_LIGHTING = 15, B200R_K_BAKE = 16, B200R_K_ATLAS = 17 };
 B200R_API void b200r_profile_enable(int on);
 B200R_API void b200r_profile_reset(void);
 B200R_API int b200r_profile_read(int kernel, double* total_ms, long long* launches);

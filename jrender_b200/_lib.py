@@ -81,6 +81,10 @@ def lib():
     L.b200r_bake_textures_softras.argtypes = [_P, _P, _P, _P, _I, _I, _I, _I, _P]
     L.b200r_bake_textures_n3mr.restype = _I
     L.b200r_bake_textures_n3mr.argtypes = [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P]
+    L.b200r_texture_atlas_softras.restype = _I
+    L.b200r_texture_atlas_softras.argtypes = [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P]
+    L.b200r_texture_atlas_n3mr.restype = _I
+    L.b200r_texture_atlas_n3mr.argtypes = [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P]
     L.b200r_set_option.restype = _I
     L.b200r_set_option.argtypes = [C.c_char_p, _I]
     _lib = L

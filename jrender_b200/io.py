@@ -1,4 +1,4 @@
-"""OBJ / MTL loading and texture baking (load-time, numpy; SURVEY.md section 8f rank 3).
+"""OBJ / MTL loading and texture baking, and the textured OBJ export (load-time; SURVEY.md section 8f rank 3).
 
 Mirrors, for the SoftRas loader:
   jrender/io/load_obj.py:9-20
@@ -10,7 +10,10 @@ Mirrors, for the SoftRas loader:
 and for the NMR loader (dr_type='n3mr'):
   jrender/io/utils/_load_obj_for_n3mr.py:11-155      (same parsing; [nf, ts, ts, ts, 3] textures, default colour 0.5)
   jrender/io/utils/load_textures.py:103-246          (the ts^3 bake with texture wrapping modes -> b200r_bake_textures_n3mr)
-Images are read with OpenCV (the reference uses skimage, which is not installed here).
+and for the export:
+  jrender/io/save_obj.py:7-84                        (.obj / .mtl / .png writer; the texture atlas is painted by
+                                                      b200r_texture_atlas_softras / _n3mr <- io/utils/create_texture_image.py)
+Images are read and written with OpenCV (the reference uses skimage, which is not installed here).
 Normal / bump maps and TBN (SSS, render2) are outside the hot-path scope.
 """
 import os
@@ -229,15 +232,134 @@ def load_obj(filename_obj, normalization=False, load_texture=False, dr_type='sof
     return v, f
 
 
-def save_obj(filename, vertices, faces):
-    """Geometry-only export (jrender/io/save_obj.py:31-84 without the texture atlas)."""
-    v = vertices.detach().cpu().numpy() if isinstance(vertices, torch.Tensor) else np.asarray(vertices)
-    f = faces.detach().cpu().numpy() if isinstance(faces, torch.Tensor) else np.asarray(faces)
+def texture_atlas(tile_vertices, textures, texture_res_out, tile_width, image_height, image_width, device=None):
+    """create_texture_image_cuda_kernel (jrender/io/utils/create_texture_image.py:3-104) through the CUDA kernels
+    b200r_texture_atlas_softras (textures [nf, R*R, 3]) / b200r_texture_atlas_n3mr (textures [nf, ts, ts, ts, 3]).
+
+    tile_vertices [nf, 3, 2]: every face's tile triangle in pixel units.  Returns the CUDA float32 image [H, W, 3] as the
+    kernel writes it (row 0 at the top, unused tiles 1).  No CPU implementation in the product (oracle/texture_atlas.py
+    is the checker)."""
+    import ctypes as C
+    from . import _lib
+    if not torch.cuda.is_available():
+        raise _lib.B200RasterError("texture-atlas export runs on the GPU (b200r_texture_atlas_*); there is no CPU fallback")
+    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+
+    def dv(x):
+        t = x.detach() if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
+        return t.to(device=dev, dtype=torch.float32).contiguous()
+    tri, tex = dv(tile_vertices), dv(textures)
+    nf = tex.shape[0]
+    if tri.shape != (nf, 3, 2):
+        raise ValueError("texture_atlas: tile_vertices must be [nf, 3, 2] for textures of %d faces" % nf)
+    if tex.dim() == 3 and tex.shape[2] == 3 and int(round(np.sqrt(tex.shape[1]))) ** 2 == tex.shape[1]:
+        fn, res, name = _lib.lib().b200r_texture_atlas_softras, int(round(np.sqrt(tex.shape[1]))), "b200r_texture_atlas_softras"
+    elif tex.dim() == 5 and tex.shape[1] == tex.shape[2] == tex.shape[3] and tex.shape[4] == 3:
+        fn, res, name = _lib.lib().b200r_texture_atlas_n3mr, tex.shape[1], "b200r_texture_atlas_n3mr"
+    else:
+        raise ValueError("texture_atlas: textures must be [nf, R*R, 3] (SoftRas) or [nf, ts, ts, ts, 3] (NMR), got %s"
+                         % (tuple(tex.shape),))
+    image = torch.empty((image_height, image_width, 3), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(fn(C.c_void_p(tri.data_ptr()), C.c_void_p(tex.data_ptr()), C.c_void_p(image.data_ptr()), nf, res,
+                      int(texture_res_out), int(tile_width), int(image_height), int(image_width),
+                      C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), name)
+    return image
+
+
+def create_texture_image(textures, texture_res=16):
+    """save_obj.py:7-29: one texture_res x texture_res tile per face in a near-square atlas.  Returns (image [H, W, 3]
+    float32 numpy, flipped vertically so that row 0 is the top of the texture as the UVs see it; uv [nf, 3, 2] float32,
+    every face's tile triangle normalised by (W - 1, H - 1)).
+
+    textures: [nf, R*R, 3] (SoftRas) or [nf, ts, ts, ts, 3] (NMR), numpy or a tensor on any device (detached).  The tile
+    row is the integer face_num // tile_width (the reference divides an int by true division there, save_obj.py:15,
+    which puts the UV triangle of every face outside the first column off the tile the kernel paints)."""
+    texture_res = int(texture_res)
+    if texture_res < 2 or texture_res == 3:
+        raise ValueError("create_texture_image: texture_res %d (must be 2 or >= 4; at 3 the tile triangle is degenerate)"
+                         % texture_res)
+    num_faces = textures.shape[0]
+    tile_width = int((num_faces - 1.) ** 0.5) + 1
+    tile_height = int((num_faces - 1.) / tile_width) + 1
+    face_nums = np.arange(num_faces)
+    column, row = face_nums % tile_width, face_nums // tile_width
+    R = texture_res
+    vertices = np.zeros((num_faces, 3, 2), np.float32)   # [:, :, UV], pixel units
+    vertices[:, 0, 0] = column * R + R / 2
+    vertices[:, 0, 1] = row * R + 1
+    vertices[:, 1, 0] = column * R + 1
+    vertices[:, 1, 1] = (row + 1) * R - 1 - 1
+    vertices[:, 2, 0] = (column + 1) * R - 1 - 1
+    vertices[:, 2, 1] = (row + 1) * R - 1 - 1
+    H, W = tile_height * R, tile_width * R
+    image = texture_atlas(vertices, textures, R, tile_width, H, W)
+    image = image.cpu().numpy() if isinstance(image, torch.Tensor) else np.asarray(image, np.float32)
+    vertices[:, :, 0] /= (W - 1)
+    vertices[:, :, 1] /= (H - 1)
+    return np.ascontiguousarray(image[::-1]), vertices
+
+
+def _host_array(x):
+    return x.detach().cpu().numpy() if isinstance(x, torch.Tensor) else np.asarray(x)
+
+
+def save_obj(filename, vertices, faces, textures=None, texture_res=16, texture_type='surface'):
+    """save_obj.py:31-84.  Without textures: the geometry only.  Surface textures ([nf, R*R, 3] or [nf, ts, ts, ts, 3]):
+    an atlas of texture_res^2 pixels per face (create_texture_image) written next to the .obj as <name>.png, <name>.mtl
+    naming it, and `vt` / `f v/vt` lines.  Vertex textures ([nv, 3]): `v x y z r g b` lines.
+
+    The textured files follow the reference's layout line for line, with two deviations: the integer tile row (see
+    create_texture_image) and no `mtllib` line for vertex colours (the reference names a .mtl it never writes, which
+    load_obj(load_texture=True) would then fail to open)."""
+    assert texture_type in ['surface', 'vertex']
+    v, f = _host_array(vertices), _host_array(faces)
     assert v.ndim == 2 and f.ndim == 2
+    if textures is None:   # the geometry-only layout this function has always written
+        with open(filename, 'w') as fh:
+            fh.write('# %s\n\n' % os.path.basename(filename))
+            for p in v:
+                fh.write('v %.8f %.8f %.8f\n' % (p[0], p[1], p[2]))
+            fh.write('\n')
+            for t in f:
+                fh.write('f %d %d %d\n' % (t[0] + 1, t[1] + 1, t[2] + 1))
+        return
+    filename_mtl = filename[:-4] + '.mtl'
+    if texture_type == 'surface':
+        import cv2
+        filename_texture = filename[:-4] + '.png'
+        material_name = 'material_1'
+        texture_image, vertices_textures = create_texture_image(textures, texture_res)
+        texture_image = (texture_image.clip(0, 1) * 255).astype('uint8')
+        if not cv2.imwrite(filename_texture, np.ascontiguousarray(texture_image[:, :, ::-1])):   # RGB -> BGR
+            raise IOError("cannot write texture image %s" % filename_texture)
+    else:
+        colors = _host_array(textures)
+        if colors.shape != (v.shape[0], 3):
+            raise ValueError("save_obj: vertex textures must be [nv, 3], got %s" % (colors.shape,))
     with open(filename, 'w') as fh:
-        fh.write('# %s\n\n' % os.path.basename(filename))
-        for p in v:
-            fh.write('v %.8f %.8f %.8f\n' % (p[0], p[1], p[2]))
+        fh.write('# %s\n' % os.path.basename(filename))
+        fh.write('#\n')
         fh.write('\n')
-        for t in f:
-            fh.write('f %d %d %d\n' % (t[0] + 1, t[1] + 1, t[2] + 1))
+        if texture_type == 'surface':
+            fh.write('mtllib %s\n\n' % os.path.basename(filename_mtl))
+            for p in v:
+                fh.write('v %.8f %.8f %.8f\n' % (p[0], p[1], p[2]))
+            fh.write('\n')
+            for p in vertices_textures.reshape((-1, 2)):
+                fh.write('vt %.8f %.8f\n' % (p[0], p[1]))
+            fh.write('\n')
+            fh.write('usemtl %s\n' % material_name)
+            for i, t in enumerate(f):
+                fh.write('f %d/%d %d/%d %d/%d\n' % (t[0] + 1, 3 * i + 1, t[1] + 1, 3 * i + 2, t[2] + 1, 3 * i + 3))
+            fh.write('\n')
+        else:
+            for p, c in zip(v, colors):
+                fh.write('v %.8f %.8f %.8f %.8f %.8f %.8f\n' % (p[0], p[1], p[2], c[0], c[1], c[2]))
+            fh.write('\n')
+            for t in f:
+                fh.write('f %d %d %d\n' % (t[0] + 1, t[1] + 1, t[2] + 1))
+    if texture_type == 'surface':
+        with open(filename_mtl, 'w') as fh:
+            fh.write('newmtl %s\n' % material_name)
+            fh.write('map_Kd %s\n' % os.path.basename(filename_texture))

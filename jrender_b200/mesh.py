@@ -230,14 +230,17 @@ class Mesh(object):
         return cls(vertices, faces, textures, texture_res, texture_type, dr_type=dr_type, with_SSS=with_SSS)
 
     def save_obj(self, filename_obj, save_texture=False, texture_res_out=16):
-        """structures/mesh.py:330-338.  Geometry only: the texture-atlas export (io/save_obj.py:9-29, a separate CUDA
-        kernel of the reference) is outside this repo's scope."""
+        """structures/mesh.py:330-338.  save_texture writes the textures too (io.save_obj): surface textures (SoftRas
+        [R*R] or NMR [ts, ts, ts]) as a texture_res_out^2-pixel-per-face atlas .png + .mtl, vertex textures as vertex
+        colours."""
         if self.batch_size != 1:
             raise ValueError('Could not save when batch size >= 1')
-        if save_texture:
-            raise NotImplementedError("save_obj(save_texture=True): texture-atlas export is not part of the rasterizer hot path")
         from .io import save_obj
-        save_obj(filename_obj, self.vertices[0], self.faces[0])
+        if save_texture:
+            save_obj(filename_obj, self.vertices[0], self.faces[0], textures=self.textures[0], texture_res=texture_res_out,
+                     texture_type=self.texture_type)
+        else:
+            save_obj(filename_obj, self.vertices[0], self.faces[0])
 
     def to(self, device):
         self._vertices = self.vertices.to(device)
