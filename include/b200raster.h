@@ -247,6 +247,22 @@ B200R_API int b200r_texture_atlas_n3mr(const float* tile_vertices, const float* 
                                        int texture_size, int texture_res_out, int tile_width, int image_height,
                                        int image_width, void* stream);
 
+/* ---- mesh voxelization -----------------------------------------------------------------------------------------
+ * Replaces jrender/renderer/utils/voxelization.py:1-57 and its four kernels (renderer/utils/cuda/voxelization.py).
+ * voxels [B, vs, vs, vs] int32 is indexed [b, c0, c1, c2] in the faces' coordinate order; 1 <= vs <= 1024.
+ *   surface: faces [B, nf, 3, 3] f32 in voxel units (already scaled).  Zeroes voxels, then sets the surface voxels of
+ *            all three axes (voxelize_sub1: integer columns (y, x), the four voxels around each accepted column) and the
+ *            voxel of every face corner (voxelize_sub2).  Bit-equal to the reference's all-columns loop in unfused
+ *            float32; a non-finite depth writes nothing.
+ *   fill:    in place: voxels becomes 1 - visible, visible = empty (== 0) voxels 6-connected through empty voxels to
+ *            the grid boundary (voxelize_sub3/4 and the host loop).  No host synchronisation; workspace of
+ *            b200r_voxelize_workspace_bytes(B, vs) bytes (0 for out-of-range arguments). */
+B200R_API size_t b200r_voxelize_workspace_bytes(int batch_size, int voxel_size);
+B200R_API int b200r_voxelize_surface(const float* faces, int32_t* voxels, int batch_size, int num_faces, int voxel_size,
+                                     void* stream);
+B200R_API int b200r_voxelize_fill(int32_t* voxels, void* workspace, size_t workspace_bytes, int batch_size, int voxel_size,
+                                  void* stream);
+
 /* ---- fused surface-mode lighting of the pre-raster stage (SURVEY.md section 8f rank 1) -------------------------
  * Replaces Lighting.execute with light_mode='surface', no normal map, no SSS, one directional light:
  *   jrender/renderer/lighting/lighting.py:186-204, ambient_lighting.py:4-9, directional_lighting.py:54-135
@@ -287,7 +303,8 @@ enum { B200R_K_FACE_SETUP = 0, B200R_K_COARSE_BIN = 1, B200R_K_SOFTRAS_FWD = 2, 
        B200R_K_TILE_ORDER = 4, B200R_K_NMR_SETUP = 5, B200R_K_NMR_FWD = 6, B200R_K_NMR_BWD_PIXEL = 7,
        B200R_K_NMR_BWD_MAPS = 8, B200R_K_SOFTRAS_BWD_FINALIZE = 9, B200R_K_NMR_PACK = 10,
        B200R_K_PROJECT_FWD = 11, B200R_K_PROJECT_BWD = 12, B200R_K_FLATTEN_LOSS = 13, B200R_K_LAPLACIAN_LOSS = 14,
-       B200R_K_LIGHTING = 15, B200R_K_BAKE = 16, B200R_K_ATLAS = 17 };
+       B200R_K_LIGHTING = 15, B200R_K_BAKE = 16, B200R_K_ATLAS = 17, B200R_K_VOXEL_SURFACE = 18,
+       B200R_K_VOXEL_FILL = 19 };
 B200R_API void b200r_profile_enable(int on);
 B200R_API void b200r_profile_reset(void);
 B200R_API int b200r_profile_read(int kernel, double* total_ms, long long* launches);

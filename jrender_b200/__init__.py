@@ -14,4 +14,5 @@ from .lighting import Lighting, AmbientLighting, DirectionalLighting  # noqa: F4
 from .renderer import Renderer  # noqa: F401
 from .preraster import project_faces  # noqa: F401
 from .loss import neg_iou_loss, LaplacianLoss, FlattenLoss  # noqa: F401
-from .io import load_obj, save_obj, create_texture_image  # noqa: F401
+from .io import load_obj, save_obj, create_texture_image, save_voxel  # noqa: F401
+from .voxelization import voxelization  # noqa: F401

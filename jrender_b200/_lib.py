@@ -85,6 +85,12 @@ def lib():
     L.b200r_texture_atlas_softras.argtypes = [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P]
     L.b200r_texture_atlas_n3mr.restype = _I
     L.b200r_texture_atlas_n3mr.argtypes = [_P, _P, _P, _I, _I, _I, _I, _I, _I, _P]
+    L.b200r_voxelize_workspace_bytes.restype = C.c_size_t
+    L.b200r_voxelize_workspace_bytes.argtypes = [_I, _I]
+    L.b200r_voxelize_surface.restype = _I
+    L.b200r_voxelize_surface.argtypes = [_P, _P, _I, _I, _I, _P]
+    L.b200r_voxelize_fill.restype = _I
+    L.b200r_voxelize_fill.argtypes = [_P, _P, C.c_size_t, _I, _I, _P]
     L.b200r_set_option.restype = _I
     L.b200r_set_option.argtypes = [C.c_char_p, _I]
     _lib = L

@@ -363,3 +363,20 @@ def save_obj(filename, vertices, faces, textures=None, texture_res=16, texture_t
         with open(filename_mtl, 'w') as fh:
             fh.write('newmtl %s\n' % material_name)
             fh.write('map_Kd %s\n' % os.path.basename(filename_texture))
+
+
+def save_voxel(filename, voxel):
+    """save_obj.py:86-94: one vertex (i / n0, j / n1, k / n2) per voxel equal to 1 of voxel [n0, n1, n2], in the
+    reference's i, j, k loop order, written as an OBJ without faces.  The reference hands save_obj a 1-D empty face array,
+    which its `len(faces.shape) == 2` assertion rejects, so it never writes a file; this writes the file that call means:
+    save_obj's geometry layout (the `#` header, the `v` lines, a blank line) with no `f` lines."""
+    v = _host_array(voxel)
+    if v.ndim != 3:
+        raise ValueError("save_voxel: voxel must be [n0, n1, n2], got %s" % (v.shape,))
+    idx = np.argwhere(v == 1)
+    vertices = (idx / np.array(v.shape, np.float64)).astype(np.float32)   # Python float division, then float32
+    with open(filename, 'w') as fh:
+        fh.write('# %s\n#\n\n' % os.path.basename(filename))
+        if len(vertices):
+            np.savetxt(fh, vertices, fmt='v %.8f %.8f %.8f')
+        fh.write('\n')

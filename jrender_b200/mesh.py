@@ -2,8 +2,8 @@
 
 Holds vertices [B,nv,3], faces [B,nf,3] and textures; lazily gathers face_vertices
 [B,nf,3,3] / face_textures -- the two tensors the rasterizer consumes.  Only the attributes the
-rasterizer path (Renderer -> Lighting -> Transform -> rasterizer) reads are mirrored; normal
-maps / TBN / SSS / voxelize are outside the hot-path scope (SURVEY.md section 8).
+rasterizer path (Renderer -> Lighting -> Transform -> rasterizer) reads are mirrored, plus export (save_obj) and
+voxelize; normal maps / TBN / SSS are outside the hot-path scope (SURVEY.md section 8).
 """
 import numpy as np
 import torch
@@ -241,6 +241,15 @@ class Mesh(object):
                      texture_type=self.texture_type)
         else:
             save_obj(filename_obj, self.vertices[0], self.faces[0])
+
+    def voxelize(self, voxel_size=32):
+        """structures/mesh.py:340-342: the face vertices mapped by v * vs / (vs - 1) + 0.5 (float32, left to right),
+        voxelized at voxel_size (jrender_b200.voxelization).  Returns int32 [B, vs, vs, vs]."""
+        from .voxelization import voxelization
+        fv = self.face_vertices.detach()
+        # a 0-dim device divisor: a CPU scalar would make torch multiply by the reciprocal instead of dividing
+        norm = fv * voxel_size / torch.tensor(float(voxel_size - 1), dtype=fv.dtype, device=fv.device) + 0.5
+        return voxelization(norm, voxel_size, False)
 
     def to(self, device):
         self._vertices = self.vertices.to(device)
