@@ -21,6 +21,21 @@ import os
 import numpy as np
 import torch
 
+from . import _lib
+
+
+def _gpu(what, device):
+    """The CUDA device a GPU-only step runs on: `device`, or the current one.  Raises when there is no GPU."""
+    if not torch.cuda.is_available():
+        raise _lib.B200RasterError("%s runs on the GPU; there is no CPU fallback" % what)
+    return torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+
+
+def _placed(x, dev, dtype=torch.float32):
+    """x (numpy array or tensor) as a contiguous `dtype` tensor on `dev`."""
+    t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
+    return t.to(device=dev, dtype=dtype).contiguous()
+
 
 def load_mtl(filename_mtl):
     """_load_obj_for_softras.py:19-40: Kd colours and map_Kd filenames per material."""
@@ -57,25 +72,14 @@ def bake_textures_for_softras(image, faces_uv, textures, is_update, device=None)
     image [H,W,3] (already flipped vertically by the caller), faces_uv [nf,3,2], textures [nf,R*R,3], is_update [nf]:
     numpy arrays or tensors; returns a CUDA float32 tensor [nf,R*R,3] (updated where is_update != 0).
     There is no CPU implementation in the product (oracle/bake.py is the checker)."""
-    import ctypes as C
-    from . import _lib
-    if not torch.cuda.is_available():
-        raise _lib.B200RasterError("texture baking runs on the GPU (b200r_bake_textures_softras); there is no CPU fallback")
-    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-
-    def dv(x, dtype):
-        t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
-        return t.to(device=dev, dtype=dtype).contiguous()
-    img, uv, upd = dv(image, torch.float32), dv(faces_uv, torch.float32), dv(is_update, torch.int32)
-    out = dv(textures, torch.float32).clone()
+    dev = _gpu("texture baking (b200r_bake_textures_softras)", device)
+    img, uv, upd = _placed(image, dev), _placed(faces_uv, dev), _placed(is_update, dev, torch.int32)
+    out = _placed(textures, dev).clone()
     nf, T = out.shape[:2]
     R = int(round(float(np.sqrt(T))))
     if R * R != T or uv.shape != (nf, 3, 2) or img.dim() != 3 or img.shape[2] != 3 or upd.shape != (nf,):
         raise ValueError("bake_textures_for_softras: image [H,W,3], faces_uv [nf,3,2], textures [nf,R*R,3], is_update [nf]")
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().b200r_bake_textures_softras(
-            C.c_void_p(img.data_ptr()), C.c_void_p(uv.data_ptr()), C.c_void_p(upd.data_ptr()), C.c_void_p(out.data_ptr()),
-            nf, R, img.shape[0], img.shape[1], C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "b200r_bake_textures_softras")
+    _lib.call("b200r_bake_textures_softras", dev, img, uv, upd, out, nf, R, img.shape[0], img.shape[1])
     return out
 
 
@@ -88,28 +92,17 @@ def bake_textures_for_n3mr(image, faces_uv, textures, is_update, texture_wrappin
     image [H,W,3] (already flipped vertically by the caller), faces_uv [nf,3,2], textures [nf,ts,ts,ts,3], is_update [nf];
     texture_wrapping 0..3 (TEXTURE_WRAPPING) or its name.  Returns a CUDA float32 tensor [nf,ts,ts,ts,3], updated where
     is_update != 0.  No CPU implementation in the product (oracle/bake.py is the checker)."""
-    import ctypes as C
-    from . import _lib
-    if not torch.cuda.is_available():
-        raise _lib.B200RasterError("texture baking runs on the GPU (b200r_bake_textures_n3mr); there is no CPU fallback")
-    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
+    dev = _gpu("texture baking (b200r_bake_textures_n3mr)", device)
     wrap = TEXTURE_WRAPPING[texture_wrapping] if isinstance(texture_wrapping, str) else int(texture_wrapping)
-
-    def dv(x, dtype):
-        t = x if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
-        return t.to(device=dev, dtype=dtype).contiguous()
-    img, uv, upd = dv(image, torch.float32), dv(faces_uv, torch.float32), dv(is_update, torch.int32)
-    out = dv(textures, torch.float32).clone()
+    img, uv, upd = _placed(image, dev), _placed(faces_uv, dev), _placed(is_update, dev, torch.int32)
+    out = _placed(textures, dev).clone()
     if out.dim() != 5 or out.shape[1] != out.shape[2] or out.shape[1] != out.shape[3] or out.shape[4] != 3:
         raise ValueError("bake_textures_for_n3mr: textures must be [nf,ts,ts,ts,3]")
     nf, ts = out.shape[0], out.shape[1]
     if uv.shape != (nf, 3, 2) or img.dim() != 3 or img.shape[2] != 3 or upd.shape != (nf,):
         raise ValueError("bake_textures_for_n3mr: image [H,W,3], faces_uv [nf,3,2], textures [nf,ts,ts,ts,3], is_update [nf]")
-    with torch.cuda.device(dev):
-        _lib.check(_lib.lib().b200r_bake_textures_n3mr(
-            C.c_void_p(img.data_ptr()), C.c_void_p(uv.data_ptr()), C.c_void_p(upd.data_ptr()), C.c_void_p(out.data_ptr()),
-            nf, ts, img.shape[0], img.shape[1], wrap, 1 if use_bilinear else 0,
-            C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "b200r_bake_textures_n3mr")
+    _lib.call("b200r_bake_textures_n3mr", dev, img, uv, upd, out, nf, ts, img.shape[0], img.shape[1], wrap,
+              1 if use_bilinear else 0)
     return out
 
 
@@ -239,31 +232,20 @@ def texture_atlas(tile_vertices, textures, texture_res_out, tile_width, image_he
     tile_vertices [nf, 3, 2]: every face's tile triangle in pixel units.  Returns the CUDA float32 image [H, W, 3] as the
     kernel writes it (row 0 at the top, unused tiles 1).  No CPU implementation in the product (oracle/texture_atlas.py
     is the checker)."""
-    import ctypes as C
-    from . import _lib
-    if not torch.cuda.is_available():
-        raise _lib.B200RasterError("texture-atlas export runs on the GPU (b200r_texture_atlas_*); there is no CPU fallback")
-    dev = torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
-
-    def dv(x):
-        t = x.detach() if isinstance(x, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(x))
-        return t.to(device=dev, dtype=torch.float32).contiguous()
-    tri, tex = dv(tile_vertices), dv(textures)
+    dev = _gpu("texture-atlas export (b200r_texture_atlas_*)", device)
+    tri, tex = _placed(tile_vertices, dev).detach(), _placed(textures, dev).detach()
     nf = tex.shape[0]
     if tri.shape != (nf, 3, 2):
         raise ValueError("texture_atlas: tile_vertices must be [nf, 3, 2] for textures of %d faces" % nf)
     if tex.dim() == 3 and tex.shape[2] == 3 and int(round(np.sqrt(tex.shape[1]))) ** 2 == tex.shape[1]:
-        fn, res, name = _lib.lib().b200r_texture_atlas_softras, int(round(np.sqrt(tex.shape[1]))), "b200r_texture_atlas_softras"
+        res, name = int(round(np.sqrt(tex.shape[1]))), "b200r_texture_atlas_softras"
     elif tex.dim() == 5 and tex.shape[1] == tex.shape[2] == tex.shape[3] and tex.shape[4] == 3:
-        fn, res, name = _lib.lib().b200r_texture_atlas_n3mr, tex.shape[1], "b200r_texture_atlas_n3mr"
+        res, name = tex.shape[1], "b200r_texture_atlas_n3mr"
     else:
         raise ValueError("texture_atlas: textures must be [nf, R*R, 3] (SoftRas) or [nf, ts, ts, ts, 3] (NMR), got %s"
                          % (tuple(tex.shape),))
     image = torch.empty((image_height, image_width, 3), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(fn(C.c_void_p(tri.data_ptr()), C.c_void_p(tex.data_ptr()), C.c_void_p(image.data_ptr()), nf, res,
-                      int(texture_res_out), int(tile_width), int(image_height), int(image_width),
-                      C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), name)
+    _lib.call(name, dev, tri, tex, image, nf, res, int(texture_res_out), int(tile_width), int(image_height), int(image_width))
     return image
 
 

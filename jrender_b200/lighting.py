@@ -7,29 +7,13 @@ including the Cook-Torrance specular branch the reference takes by default
 (Mesh.with_specular defaults to True, structures/mesh.py:74).  Normal-mapped meshes
 (surface_ResNormals), SSS and the Gbuffer debug modes are not mirrored.
 """
-import ctypes as C
-
 import torch
 from torch import nn
 import torch.nn.functional as F
 
 from . import _lib
-
-
-_CONST = {}
-
-
-def _t(x, like):
-    """Python constants (light colours / directions) live on the device once per (value, device):
-    building them per call is a pageable H2D copy, which stalls the stream and cannot be captured
-    in a CUDA graph."""
-    if isinstance(x, torch.Tensor):
-        return x.to(device=like.device, dtype=torch.float32)
-    key = (repr(x), str(like.device))
-    t = _CONST.get(key)
-    if t is None:
-        t = _CONST[key] = torch.tensor(x, dtype=torch.float32, device=like.device)
-    return t
+from ._lib import _f3
+from .transform import _t
 
 
 def ambient_lighting(light, light_intensity=0.5, light_color=(1, 1, 1)):
@@ -118,22 +102,11 @@ def directional_lighting(diffuseLight, specularLight, normals, light_intensity=0
     return [diffuseLight, specularLight]
 
 
-def _f3(x):
-    """3 host floats as a ctypes array (light colours / direction are Python constants in the reference's API)."""
-    if isinstance(x, torch.Tensor):
-        x = x.detach().cpu().tolist()
-    x = [float(v) for v in x]
-    if len(x) != 3:
-        raise ValueError("expected 3 components, got %r" % (x,))
-    return (C.c_float * 3)(*x)
-
-
 class _FusedSurfaceLighting(torch.autograd.Function):
     """clamp(textures * diffuse + specular, 0, 1) with diffuse / specular from the face normals: b200r_surface_lighting_*."""
 
     @staticmethod
     def forward(ctx, vertices, textures, faces, metallic, roughness, eye, params):
-        dev = vertices.device
         v = vertices.contiguous()
         tx = textures.contiguous()
         B, nf = tx.shape[0], tx.shape[1]
@@ -143,11 +116,7 @@ class _FusedSurfaceLighting(torch.autograd.Function):
         amb_i, amb_c, dir_i, dir_c, direction, with_spec = params
         args = (B, v.shape[0], faces.shape[0], 0 if eye is None else eye.shape[0], v.shape[1], nf, T, Tm,
                 float(amb_i), _f3(amb_c), float(dir_i), _f3(dir_c), _f3(direction), int(bool(with_spec)))
-        with torch.cuda.device(dev):
-            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())   # noqa: E731
-            _lib.check(_lib.lib().b200r_surface_lighting_forward(p(v), p(faces), p(tx), p(metallic), p(roughness), p(eye), p(out), *args, st),
-                       "b200r_surface_lighting_forward")
+        _lib.call("b200r_surface_lighting_forward", v.device, v, faces, tx, metallic, roughness, eye, out, *args)
         ctx.save_for_backward(v, tx, faces, metallic, roughness, eye)
         ctx.args = args
         return out
@@ -155,15 +124,10 @@ class _FusedSurfaceLighting(torch.autograd.Function):
     @staticmethod
     def backward(ctx, grad_out):
         v, tx, faces, metallic, roughness, eye = ctx.saved_tensors
-        dev = v.device
         g = grad_out.contiguous()
         gt = torch.empty_like(tx)
         gv = torch.empty_like(v) if ctx.needs_input_grad[0] else None
-        with torch.cuda.device(dev):
-            st = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-            p = lambda t: C.c_void_p(0 if t is None else t.data_ptr())   # noqa: E731
-            _lib.check(_lib.lib().b200r_surface_lighting_backward(p(v), p(faces), p(tx), p(metallic), p(roughness), p(eye), p(g), p(gt), p(gv),
-                                                                  *ctx.args, st), "b200r_surface_lighting_backward")
+        _lib.call("b200r_surface_lighting_backward", v.device, v, faces, tx, metallic, roughness, eye, g, gt, gv, *ctx.args)
         return gv, (gt if ctx.needs_input_grad[1] else None), None, None, None, None, None
 
 

@@ -4,8 +4,6 @@ neg_iou_loss  (iou_loss.py:1-5), LaplacianLoss (laplacian_loss.py:5-36, stored a
 neighbour table instead of the reference's dense nv x nv matrix -- same values), FlattenLoss
 (flatten_loss.py:5-79, edge table built with a dictionary instead of the O(E*F) scan).
 """
-import ctypes as C
-
 import numpy as np
 import torch
 from torch import nn
@@ -14,31 +12,26 @@ from . import _lib
 
 
 class _FusedMeshLoss(torch.autograd.Function):
-    """loss [B] and d loss / d vertices from ONE launch of csrc/mesh_loss_api.cu; the backward is a scale."""
+    """loss [B] and d loss / d vertices from ONE launch of csrc/mesh_loss_api.cu; the backward is a scale.
+    `name`(vertices, *tables, loss, grad, batch_size, num_vertices, *scalars, stream) is the entry point."""
 
     @staticmethod
-    def forward(ctx, vertices, launch):
+    def forward(ctx, vertices, name, tables, scalars):
         v = vertices.contiguous()
-        dev = v.device
-        with torch.cuda.device(dev):
-            loss = torch.empty((v.shape[0],), dtype=torch.float32, device=dev)
-            grad = torch.empty_like(v)
-            launch(v, loss, grad, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+        loss = torch.empty((v.shape[0],), dtype=torch.float32, device=v.device)
+        grad = torch.empty_like(v)
+        _lib.call(name, v.device, v, *tables, loss, grad, v.shape[0], v.shape[1], *scalars)
         ctx.save_for_backward(grad)
         return loss
 
     @staticmethod
     def backward(ctx, grad_loss):
         (grad,) = ctx.saved_tensors
-        return grad * grad_loss[:, None, None], None
+        return grad * grad_loss[:, None, None], None, None, None
 
 
 def _fusable(x):
     return x.is_cuda and x.dtype == torch.float32 and x.dim() == 3 and x.shape[2] == 3 and 0 < x.shape[0] <= 65535
-
-
-def _p(t):
-    return C.c_void_p(t.data_ptr())
 
 
 def neg_iou_loss(predict, target):
@@ -82,13 +75,7 @@ class LaplacianLoss(nn.Module):
     def forward(self, x):
         batch_size = x.shape[0]
         if self.fused and _fusable(x) and x.shape[1] == self.nv and self.nbr32.device == x.device:
-            L = _lib.lib()
-            maxdeg = self.nbr_w.shape[1]
-
-            def launch(v, loss, grad, stream):
-                _lib.check(L.b200r_laplacian_loss(_p(v), _p(self.nbr32), _p(self.nbr_w), _p(self.diag), _p(loss), _p(grad),
-                                                  v.shape[0], self.nv, maxdeg, stream), "b200r_laplacian_loss")
-            y = _FusedMeshLoss.apply(x, launch)
+            y = _FusedMeshLoss.apply(x, "b200r_laplacian_loss", (self.nbr32, self.nbr_w, self.diag), (self.nbr_w.shape[1],))
             return y.sum() / batch_size if self.average else y
         xn = torch.index_select(x, 1, self.nbr).view(batch_size, self.nv, -1, x.shape[2])
         y = x * self.diag[None, :, None] + (xn * self.nbr_w[None, :, :, None]).sum(2)
@@ -134,14 +121,7 @@ class FlattenLoss(nn.Module):
         # the kernel dereferences the module's index buffers: they must live on the input's device, otherwise the
         # index_select path below raises torch's own device-mismatch error
         if self.fused and _fusable(vertices) and self.e32.device == vertices.device:
-            L = _lib.lib()
-            E = int(self.v0s.shape[0])
-
-            def launch(v, loss, grad, stream):
-                _lib.check(L.b200r_flatten_loss(_p(v), _p(self.e32[0]), _p(self.e32[1]), _p(self.e32[2]), _p(self.e32[3]),
-                                                _p(loss), _p(grad), v.shape[0], v.shape[1], E, float(eps), stream),
-                           "b200r_flatten_loss")
-            loss = _FusedMeshLoss.apply(vertices, launch)
+            loss = _FusedMeshLoss.apply(vertices, "b200r_flatten_loss", tuple(self.e32), (int(self.v0s.shape[0]), float(eps)))
             return loss.sum() / batch_size if self.average else loss
         v0s = torch.index_select(vertices, 1, self.v0s)   # backward = index_add (graph-capturable)
         v1s = torch.index_select(vertices, 1, self.v1s)

@@ -9,8 +9,6 @@ Mirrors (same names, arguments, defaults, return conventions):
 Compute: libb200raster.so (b200r_nmr_forward / b200r_nmr_backward, hand-written sm_90a
 kernels); PyTorch owns memory, the stream and autograd glue.  CUDA tensors only.
 """
-import ctypes as C
-
 import numpy as np
 import torch
 from torch import nn
@@ -23,10 +21,6 @@ DEFAULT_NEAR = 0.1
 DEFAULT_FAR = 100
 DEFAULT_EPS = 1e-4
 DEFAULT_BACKGROUND_COLOR = (0, 0, 0)
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else None
 
 
 class _RasterizeOp(torch.autograd.Function):
@@ -45,32 +39,28 @@ class _RasterizeOp(torch.autograd.Function):
         ts = int(tx.shape[2]) if rgb else 0
         bg = fn.background_color
         bg2d = None
-        bg_host = (C.c_float * 3)(0.0, 0.0, 0.0)
+        bg_host = _lib._f3((0.0, 0.0, 0.0))
         if rgb and bg is not None:
             bgt = torch.as_tensor(bg, dtype=torch.float32)
             if bgt.dim() == 1:
-                bg_host = (C.c_float * 3)(*[float(x) for x in bgt.tolist()])
+                bg_host = _lib._f3(bgt)
             else:
                 bg2d = bgt.to(dev)          # per-batch background (n3mr.py:141-142): mixed below
-        with torch.cuda.device(dev):
-            face_index_map = torch.empty((B, H, H), dtype=torch.int32, device=dev)
-            weight_map = torch.empty((B, H, H, 3), dtype=torch.float32, device=dev)
-            depth_map = torch.empty((B, H, H), dtype=torch.float32, device=dev)
-            rgb_map = torch.empty((B, H, H, 3), dtype=torch.float32, device=dev) if rgb else None
-            sidx = torch.empty((B, H, H, 8), dtype=torch.int32, device=dev) if rgb else None
-            swgt = torch.empty((B, H, H, 8), dtype=torch.float32, device=dev) if rgb else None
-            alpha_map = torch.empty((B, H, H), dtype=torch.float32, device=dev) if alpha else None
-            face_inv_map = torch.empty((B, H, H, 3, 3), dtype=torch.float32, device=dev) if depth_req else None
-            ws_bytes = L.b200r_nmr_workspace_bytes(B, nf, H)
-            workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-            f32 = np.float32
-            rc = L.b200r_nmr_forward(
-                _ptr(fc), _ptr(tx), _ptr(face_index_map), _ptr(weight_map), _ptr(depth_map), _ptr(rgb_map),
-                _ptr(alpha_map), _ptr(sidx), _ptr(swgt), _ptr(face_inv_map), _ptr(workspace), ws_bytes,
-                B, nf, ts, H, float(f32(fn.near)), float(f32(fn.far)), float(f32(fn.eps)),
-                C.cast(bg_host, C.c_void_p), int(rgb), int(alpha), int(depth_req),
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        _lib.check(rc, "b200r_nmr_forward")
+        face_index_map = torch.empty((B, H, H), dtype=torch.int32, device=dev)
+        weight_map = torch.empty((B, H, H, 3), dtype=torch.float32, device=dev)
+        depth_map = torch.empty((B, H, H), dtype=torch.float32, device=dev)
+        rgb_map = torch.empty((B, H, H, 3), dtype=torch.float32, device=dev) if rgb else None
+        sidx = torch.empty((B, H, H, 8), dtype=torch.int32, device=dev) if rgb else None
+        swgt = torch.empty((B, H, H, 8), dtype=torch.float32, device=dev) if rgb else None
+        alpha_map = torch.empty((B, H, H), dtype=torch.float32, device=dev) if alpha else None
+        face_inv_map = torch.empty((B, H, H, 3, 3), dtype=torch.float32, device=dev) if depth_req else None
+        ws_bytes = L.b200r_nmr_workspace_bytes(B, nf, H)
+        workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        f32 = np.float32
+        _lib.call("b200r_nmr_forward", dev,
+                  fc, tx, face_index_map, weight_map, depth_map, rgb_map, alpha_map, sidx, swgt, face_inv_map,
+                  workspace, ws_bytes, B, nf, ts, H, float(f32(fn.near)), float(f32(fn.far)), float(f32(fn.eps)),
+                  bg_host, int(rgb), int(alpha), int(depth_req))
         if bg2d is not None:
             mask = (face_index_map >= 0).float().unsqueeze(-1)
             rgb_map = rgb_map * mask + (1 - mask) * bg2d[:, None, None, :]
@@ -95,27 +85,22 @@ class _RasterizeOp(torch.autograd.Function):
             [None if is_none else next(it) for is_none in ctx.none_mask]
         B, nf, ts, H = ctx.dims
         rgb, alpha, depth_req = ctx.flags
-        L = _lib.lib()
         dev = fc.device
 
         def prep(g, like):
             if g is None:
                 return torch.zeros_like(like)       # n3mr.py:40-52: missing upstream gradients are zeros
             return g.contiguous().float()
-        with torch.cuda.device(dev):
-            g_rgb = prep(grad_rgb_map, rgb_map) if rgb else None
-            g_a = prep(grad_alpha_map, alpha_map) if alpha else None
-            g_d = prep(grad_depth_map, depth_map) if depth_req else None
-            grad_faces = torch.empty_like(fc)
-            grad_textures = torch.empty_like(tx) if rgb else None
-            sc_bytes = L.b200r_nmr_backward_scratch_bytes(B, H) if (rgb or alpha) else 0
-            scratch = torch.empty((sc_bytes,), dtype=torch.uint8, device=dev) if sc_bytes else None
-            rc = L.b200r_nmr_backward(
-                _ptr(fc), _ptr(face_index_map), _ptr(weight_map), _ptr(depth_map), _ptr(rgb_map), _ptr(alpha_map),
-                _ptr(sidx), _ptr(swgt), _ptr(face_inv_map), _ptr(g_rgb), _ptr(g_a), _ptr(g_d),
-                _ptr(grad_faces), _ptr(grad_textures), _ptr(scratch), sc_bytes, B, nf, ts, H, ctx.eps,
-                int(rgb), int(alpha), int(depth_req), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        _lib.check(rc, "b200r_nmr_backward")
+        g_rgb = prep(grad_rgb_map, rgb_map) if rgb else None
+        g_a = prep(grad_alpha_map, alpha_map) if alpha else None
+        g_d = prep(grad_depth_map, depth_map) if depth_req else None
+        grad_faces = torch.empty_like(fc)
+        grad_textures = torch.empty_like(tx) if rgb else None
+        sc_bytes = _lib.lib().b200r_nmr_backward_scratch_bytes(B, H) if (rgb or alpha) else 0
+        scratch = torch.empty((sc_bytes,), dtype=torch.uint8, device=dev) if sc_bytes else None
+        _lib.call("b200r_nmr_backward", dev,
+                  fc, face_index_map, weight_map, depth_map, rgb_map, alpha_map, sidx, swgt, face_inv_map, g_rgb, g_a, g_d,
+                  grad_faces, grad_textures, scratch, sc_bytes, B, nf, ts, H, ctx.eps, int(rgb), int(alpha), int(depth_req))
         return grad_faces, grad_textures, None
 
 

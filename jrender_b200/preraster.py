@@ -12,27 +12,16 @@ backward), replacing the reference's chain of tensor ops
 here for camera_mode 'look_at' / 'look' on CUDA tensors; everything else keeps the op-by-op
 PyTorch mirror.  There is no CPU path: CPU tensors raise.
 """
-import ctypes as C
 import math
 
 import numpy as np
 import torch
 
 from . import _lib
+from ._lib import _f3
 
 CAM_MODES = {'look_at': 0, 'look_right': 1, 'look_left': 2}
 PROJECTIONS = {'perspective': 0, 'orthogonal': 1}
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
-
-
-def _f3(x):
-    a = np.asarray(x, dtype=np.float32).reshape(-1)
-    if a.shape[0] != 3:
-        raise ValueError("expected 3 components, got %r" % (x,))
-    return (C.c_float * 3)(*[float(v) for v in a])
 
 
 def perspective_width(angle):
@@ -43,17 +32,12 @@ def perspective_width(angle):
 class _ProjectFacesOp(torch.autograd.Function):
     @staticmethod
     def forward(ctx, vertices, faces, eye, cfg):
-        L = _lib.lib()
         v = vertices.contiguous()
         B, nf = cfg["B"], faces.shape[1]
-        dev = v.device
-        with torch.cuda.device(dev):
-            out = torch.empty((B, nf, 3, 3), dtype=torch.float32, device=dev)
-            rc = L.b200r_project_faces_forward(
-                _ptr(v), _ptr(faces), _ptr(eye), _ptr(out), cfg["at"], cfg["up"], cfg["width"], cfg["mode"], cfg["proj"],
-                B, v.shape[1], nf, v.shape[0], faces.shape[0], eye.shape[0],
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        _lib.check(rc, "b200r_project_faces_forward")
+        out = torch.empty((B, nf, 3, 3), dtype=torch.float32, device=v.device)
+        _lib.call("b200r_project_faces_forward", v.device,
+                  v, faces, eye, out, cfg["at"], cfg["up"], cfg["width"], cfg["mode"], cfg["proj"],
+                  B, v.shape[1], nf, v.shape[0], faces.shape[0], eye.shape[0])
         ctx.cfg = cfg
         ctx.save_for_backward(v, faces, eye)
         return out
@@ -62,18 +46,13 @@ class _ProjectFacesOp(torch.autograd.Function):
     def backward(ctx, grad_out):
         v, faces, eye = ctx.saved_tensors
         cfg = ctx.cfg
-        L = _lib.lib()
         g = grad_out.contiguous()
         if g.dtype != torch.float32:
             g = g.float()
-        dev = v.device
-        with torch.cuda.device(dev):
-            gv = torch.empty_like(v)
-            rc = L.b200r_project_faces_backward(
-                _ptr(v), _ptr(faces), _ptr(eye), _ptr(g), _ptr(gv), cfg["at"], cfg["up"], cfg["width"], cfg["mode"],
-                cfg["proj"], cfg["B"], v.shape[1], faces.shape[1], v.shape[0], faces.shape[0], eye.shape[0],
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        _lib.check(rc, "b200r_project_faces_backward")
+        gv = torch.empty_like(v)
+        _lib.call("b200r_project_faces_backward", v.device,
+                  v, faces, eye, g, gv, cfg["at"], cfg["up"], cfg["width"], cfg["mode"],
+                  cfg["proj"], cfg["B"], v.shape[1], faces.shape[1], v.shape[0], faces.shape[0], eye.shape[0])
         return gv, None, None, None
 
 
@@ -128,5 +107,5 @@ def project_faces(vertices, faces, eye, camera_mode='look_at', at=(0, 0, 0), dir
         raise ValueError("project_faces supports camera_mode 'look_at' and 'look'")
     cfg = {"B": B, "at": a, "up": _f3(up), "mode": mode,
            "proj": PROJECTIONS['perspective' if perspective else 'orthogonal'],
-           "width": C.c_float(perspective_width(viewing_angle) if perspective else float(viewing_scale))}
+           "width": perspective_width(viewing_angle) if perspective else float(viewing_scale)}
     return _ProjectFacesOp.apply(vertices, f, e, cfg)

@@ -9,7 +9,6 @@ The compute is done by libb200raster.so (hand-written sm_90a kernels) through th
 in include/b200raster.h; PyTorch only owns device memory, the stream and autograd glue.
 There is no CPU path: tensors must live on a CUDA device.
 """
-import ctypes as C
 import math
 
 import numpy as np
@@ -22,10 +21,6 @@ FUNC_DIST_MAP = {'hard': 0, 'barycentric': 1, 'euclidean': 2}   # soft_rasterize
 FUNC_RGB_MAP = {'hard': 0, 'softmax': 1, 'none': 2}             # :40
 FUNC_ALPHA_MAP = {'hard': 0, 'sum': 1, 'prod': 2}               # :41
 FUNC_MAP_SAMPLE = {'surface': 0, 'vertex': 1}                   # :42
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
 
 
 def _check_inputs(face_vertices, textures):
@@ -63,31 +58,23 @@ class _SoftRasterizeOp(torch.autograd.Function):
         H = int(fn.image_size)
         K = int(fn.max_faces_id)
         dev = fv.device
-        with torch.cuda.device(dev):
-            soft_colors = torch.empty((B, 4, H, H), dtype=torch.float32, device=dev)
-            aggrs_info = torch.empty((B, 2, H, H), dtype=torch.float32, device=dev)
-            faces_id_buffer = torch.empty((B, K, H, H), dtype=torch.int32, device=dev)
-            faces_info = torch.empty((B, nf, 27), dtype=torch.float32, device=dev) if fn.return_faces_info else None
-            # state: records + gradient accumulator, kept for the backward; workspace: binning scratch, released (back to
-            # the caching allocator) as soon as this call returns -- it is not part of the saved state
-            st_bytes = L.b200r_softras_state_bytes(B, nf)
-            state = torch.empty((st_bytes,), dtype=torch.uint8, device=dev)
-            ws_bytes = L.b200r_softras_workspace_bytes(B, nf, H)
-            workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-            scal = fn._scalars(B, nf, T)
-            pooled = None
-            if getattr(fn, "pool2x2", False):   # anti-aliasing epilogue: the forward also writes the 2x2 means
-                pooled = torch.empty((B, 4, H // 2, H // 2), dtype=torch.float32, device=dev)
-                rc = L.b200r_softras_forward_aa(
-                    _ptr(fv), _ptr(tx), _ptr(soft_colors), _ptr(pooled), _ptr(aggrs_info), _ptr(faces_id_buffer),
-                    _ptr(faces_info) if faces_info is not None else None, _ptr(state), st_bytes, _ptr(workspace), ws_bytes,
-                    *scal, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-            else:
-                rc = L.b200r_softras_forward(
-                    _ptr(fv), _ptr(tx), _ptr(soft_colors), _ptr(aggrs_info), _ptr(faces_id_buffer),
-                    _ptr(faces_info) if faces_info is not None else None, _ptr(state), st_bytes, _ptr(workspace), ws_bytes,
-                    *scal, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        _lib.check(rc, "b200r_softras_forward")
+        soft_colors = torch.empty((B, 4, H, H), dtype=torch.float32, device=dev)
+        aggrs_info = torch.empty((B, 2, H, H), dtype=torch.float32, device=dev)
+        faces_id_buffer = torch.empty((B, K, H, H), dtype=torch.int32, device=dev)
+        faces_info = torch.empty((B, nf, 27), dtype=torch.float32, device=dev) if fn.return_faces_info else None
+        # state: records + gradient accumulator, kept for the backward; workspace: binning scratch, released (back to
+        # the caching allocator) as soon as this call returns -- it is not part of the saved state
+        st_bytes = L.b200r_softras_state_bytes(B, nf)
+        state = torch.empty((st_bytes,), dtype=torch.uint8, device=dev)
+        ws_bytes = L.b200r_softras_workspace_bytes(B, nf, H)
+        workspace = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+        scal = fn._scalars(B, nf, T)
+        pooled = None
+        if getattr(fn, "pool2x2", False):   # anti-aliasing epilogue: the forward also writes the 2x2 means
+            pooled = torch.empty((B, 4, H // 2, H // 2), dtype=torch.float32, device=dev)
+        _lib.call("b200r_softras_forward" if pooled is None else "b200r_softras_forward_aa", dev,
+                  fv, tx, soft_colors, *(() if pooled is None else (pooled,)), aggrs_info, faces_id_buffer, faces_info,
+                  state, st_bytes, workspace, ws_bytes, *scal)
         ctx.pool2x2 = pooled is not None
         ctx.scal = scal
         ctx.st_bytes = st_bytes
@@ -113,20 +100,14 @@ class _SoftRasterizeOp(torch.autograd.Function):
         if grad_soft_colors is None:   # soft_colors did not take part in the loss
             return None, None, None
         fv, tx, soft_colors, aggrs_info, faces_id_buffer, state = ctx.saved_tensors
-        L = _lib.lib()
-        dev = fv.device
         g = grad_soft_colors.contiguous()
         if g.dtype != torch.float32:
             g = g.float()
-        with torch.cuda.device(dev):
-            grad_faces = torch.empty_like(fv)
-            grad_textures = torch.empty_like(tx)
-            call = L.b200r_softras_backward_aa if ctx.pool2x2 else L.b200r_softras_backward   # g: pooled gradient under AA
-            rc = call(
-                _ptr(fv), _ptr(tx), _ptr(soft_colors), _ptr(aggrs_info), _ptr(faces_id_buffer),
-                _ptr(state), ctx.st_bytes, _ptr(g), _ptr(grad_faces), _ptr(grad_textures),
-                *ctx.scal, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
-        _lib.check(rc, "b200r_softras_backward")
+        grad_faces = torch.empty_like(fv)
+        grad_textures = torch.empty_like(tx)
+        _lib.call("b200r_softras_backward_aa" if ctx.pool2x2 else "b200r_softras_backward", fv.device,   # g: pooled under AA
+                  fv, tx, soft_colors, aggrs_info, faces_id_buffer, state, ctx.st_bytes, g, grad_faces, grad_textures,
+                  *ctx.scal)
         return grad_faces, grad_textures, None
 
 

@@ -5,8 +5,6 @@ surface voxels of all three axes and of the face corners, and b200r_voxelize_fil
 6-connected through empty voxels to the grid boundary.  Both run on the caller's current stream with no host
 synchronisation, so a call can be captured in a CUDA graph.
 """
-import ctypes as C
-
 import torch
 
 from . import _lib
@@ -18,10 +16,7 @@ def voxelize_surface(faces, size):
     faces = faces.detach().contiguous()
     B, nf = faces.shape[0], faces.shape[1]
     voxels = torch.empty((B, size, size, size), dtype=torch.int32, device=faces.device)
-    with torch.cuda.device(faces.device):
-        _lib.check(_lib.lib().b200r_voxelize_surface(
-            C.c_void_p(faces.data_ptr()), C.c_void_p(voxels.data_ptr()), B, nf, size,
-            C.c_void_p(torch.cuda.current_stream(faces.device).cuda_stream)), "b200r_voxelize_surface")
+    _lib.call("b200r_voxelize_surface", faces.device, faces, voxels, B, nf, size)
     return voxels
 
 
@@ -34,13 +29,9 @@ def voxelize_fill(voxels):
     B, vs = voxels.shape[0], voxels.shape[1]
     if voxels.shape[1:] != (vs, vs, vs):
         raise ValueError("voxelize_fill: voxels must be [B, vs, vs, vs], got %s" % (tuple(voxels.shape),))
-    L = _lib.lib()
-    nbytes = L.b200r_voxelize_workspace_bytes(B, vs)
+    nbytes = _lib.lib().b200r_voxelize_workspace_bytes(B, vs)
     workspace = torch.empty(max(nbytes, 1), dtype=torch.uint8, device=voxels.device)
-    with torch.cuda.device(voxels.device):
-        _lib.check(L.b200r_voxelize_fill(C.c_void_p(voxels.data_ptr()), C.c_void_p(workspace.data_ptr()), nbytes, B, vs,
-                                         C.c_void_p(torch.cuda.current_stream(voxels.device).cuda_stream)),
-                   "b200r_voxelize_fill")
+    _lib.call("b200r_voxelize_fill", voxels.device, voxels, workspace, nbytes, B, vs)
     return voxels
 
 

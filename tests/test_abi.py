@@ -35,6 +35,65 @@ def test_library_exports_every_declared_symbol(lib):
         assert hasattr(lib, s), "libb200raster.so does not export %s" % s
 
 
+def declared_arg_counts():
+    src = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "b200raster.h")).read(), flags=re.S)
+    return {name: 0 if params.strip() in ("", "void") else params.count(",") + 1
+            for name, params in re.findall(r"B200R_API\s+[\w\s\*]+?\b(b200r_\w+)\s*\(([^)]*)\)", src)}
+
+
+def test_every_declaration_is_bound_from_the_header(lib):
+    counts = declared_arg_counts()
+    assert sorted(counts) == declared_symbols() and len(counts) >= 31
+    for name, n in counts.items():
+        argtypes = getattr(lib, name).argtypes
+        assert argtypes is not None and len(argtypes) == n, (name, argtypes, n)
+
+
+def test_bindings_match_the_c_types(lib):
+    P, I, F, Z = C.c_void_p, C.c_int, C.c_float, C.c_size_t
+    want = {
+        "b200r_voxelize_fill": (I, [P, P, Z, I, I, P]),
+        "b200r_nmr_backward": (I, [P] * 15 + [Z, I, I, I, I, F, I, I, I, P]),
+        "b200r_softras_workspace_bytes": (Z, [I, I, I]),
+        "b200r_profile_enable": (None, [I]),
+        "b200r_profile_read": (I, [I, P, P]),
+        "b200r_version": (C.c_char_p, []),
+        "b200r_launch_count": (C.c_ulonglong, []),
+        "b200r_set_option": (I, [C.c_char_p, I]),
+    }
+    for name, (restype, argtypes) in want.items():
+        fn = getattr(lib, name)
+        assert (fn.restype, fn.argtypes) == (restype, argtypes), name
+
+
+def test_header_parser_rejects_what_it_cannot_bind():
+    from jrender_b200 import _lib
+    sigs = _lib.parse_header("/* B200R_API int b200r_commented(double x); */\n#define B200R_API\n"
+                             "B200R_API const char* b200r_a(void);\n"
+                             "B200R_API void b200r_b(const float* p, const int32_t* q, unsigned long long n, void* s);\n")
+    assert sigs == {"b200r_a": (C.c_char_p, []),
+                    "b200r_b": (None, [C.c_void_p, C.c_void_p, C.c_ulonglong, C.c_void_p])}
+    for bad in ("B200R_API int b200r_x(double d, void* stream);",      # unknown argument type
+                "B200R_API double b200r_x(int n);",                    # unknown return type
+                "B200R_API int b200r_x(int (*cb)(int), void* stream);"):   # a declaration the parser cannot read
+        with pytest.raises(_lib.B200RasterError):
+            _lib.parse_header(bad)
+
+
+@pytest.mark.gpu
+def test_failing_call_names_the_entry_point(cuda_device):
+    """The anti-aliased forward rejects an odd supersampled size; the error names the function that was called."""
+    import torch
+    from jrender_b200 import B200RasterError, SoftRasterizeFunction
+    fn = SoftRasterizeFunction(image_size=65)
+    fn.pool2x2 = True
+    fv = torch.rand(1, 8, 3, 3, device=cuda_device)
+    tex = torch.rand(1, 8, 1, 3, device=cuda_device)
+    with pytest.raises(B200RasterError) as e:
+        fn(fv, tex)
+    assert str(e.value).startswith("b200r_softras_forward_aa failed"), str(e.value)
+
+
 def test_version_and_workspace_size(lib):
     assert b"sm_90a" in lib.b200r_version()
     assert lib.b200r_softras_workspace_bytes(0, 10, 64) == 0

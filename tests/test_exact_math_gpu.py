@@ -1,8 +1,6 @@
 """GPU check that csrc/exact_math.cuh reproduces the plain IEEE expressions bit for bit:
 fast_div == a / b (nvcc's own division), f2d_mid == (double)x, d2f_mid == (float)d (including
 exact round-to-even ties), sigmoid_tail and alpha_prod == the reference's double expressions."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -12,13 +10,10 @@ pytestmark = pytest.mark.gpu
 def _run(a, b):
     import torch
     from jrender_b200 import _lib
-    L = _lib.lib()
     ta = torch.from_numpy(a).cuda()
     tb = torch.from_numpy(b).cuda()
     mm = torch.zeros(7, dtype=torch.int32, device="cuda")
-    rc = L.b200r_debug_exact_math(C.c_void_p(ta.data_ptr()), C.c_void_p(tb.data_ptr()), a.size,
-                                  C.c_void_p(mm.data_ptr()), C.c_void_p(torch.cuda.current_stream().cuda_stream))
-    _lib.check(rc, "b200r_debug_exact_math")
+    _lib.call("b200r_debug_exact_math", mm.device, ta, tb, a.size, mm)
     return mm.cpu().numpy()
 
 

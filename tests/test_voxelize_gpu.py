@@ -4,7 +4,6 @@ The surface kernel and the fill are bit-equal to the numpy oracle (oracle/voxeli
 in unfused float32, and a BFS).  Against the reference's own kernels (tests/golden/ref_voxel_gpu_*.npz, built with a*b+c
 contraction) a differing surface voxel must be one a marginal pair can set, as in tests/test_voxelize_cpu.py.
 """
-import ctypes as C
 import importlib
 import os
 
@@ -183,9 +182,7 @@ def test_no_writes_outside_the_grid(cuda_device):
     n = B * vs ** 3
     big = torch.full((n + 2 * 4096,), -7, dtype=torch.int32, device=cuda_device)
     view = big[4096:4096 + n].view(B, vs, vs, vs)
-    L = _lib.lib()
-    _lib.check(L.b200r_voxelize_surface(C.c_void_p(faces.data_ptr()), C.c_void_p(view.data_ptr()), B, faces.shape[1], vs,
-                                        C.c_void_p(torch.cuda.current_stream().cuda_stream)), "surface")
+    _lib.call("b200r_voxelize_surface", cuda_device, faces, view, B, faces.shape[1], vs)
     jv.voxelize_fill(view)
     torch.cuda.synchronize()
     assert (big[:4096] == -7).all() and (big[4096 + n:] == -7).all()
