@@ -271,8 +271,10 @@ B200R_API int b200r_voxelize_fill(int32_t* voxels, void* workspace, size_t works
  * vertices [vertices_batch, nv, 3] world space, faces [faces_batch, nf, 3] int32, textures / out_textures
  * [B, nf, T, 3] (T = texture_res^2, or ts^3 for n3mr), metallic / roughness [B, nf, Tm] or NULL, eye [eye_batch, 3]
  * (eye_batch 0: none).  Batches of 1 broadcast.  ambient_color, directional_color, direction: HOST pointers to 3 floats
- * (direction already normalised).  backward overwrites grad_textures [B, nf, T, 3] and grad_vertices
- * [vertices_batch, nv, 3] (NULL: not needed). */
+ * (direction already normalised).  backward overwrites grad_textures [B, nf, T, 3], grad_vertices
+ * [vertices_batch, nv, 3], and grad_metallic / grad_roughness [B, nf, Tm] (each NULL: not needed).  A material gradient
+ * is the gradient of the face's mean material value spread evenly over its Tm texels; it is 0 where the Cook-Torrance
+ * branch is off (with_specular 0 or no eye).  Material gradients need metallic, roughness and Tm > 0 (else B200R_EINVAL). */
 B200R_API int b200r_surface_lighting_forward(const float* vertices, const int32_t* faces, const float* textures, const float* metallic,
                                              const float* roughness, const float* eye, float* out_textures, int B, int vertices_batch,
                                              int faces_batch, int eye_batch, int nv, int nf, int T, int Tm, float ambient_intensity,
@@ -280,10 +282,10 @@ B200R_API int b200r_surface_lighting_forward(const float* vertices, const int32_
                                              const float* direction, int with_specular, void* stream);
 B200R_API int b200r_surface_lighting_backward(const float* vertices, const int32_t* faces, const float* textures, const float* metallic,
                                               const float* roughness, const float* eye, const float* grad_out, float* grad_textures,
-                                              float* grad_vertices, int B, int vertices_batch, int faces_batch, int eye_batch, int nv,
-                                              int nf, int T, int Tm, float ambient_intensity, const float* ambient_color,
-                                              float directional_intensity, const float* directional_color, const float* direction,
-                                              int with_specular, void* stream);
+                                              float* grad_vertices, float* grad_metallic, float* grad_roughness, int B,
+                                              int vertices_batch, int faces_batch, int eye_batch, int nv, int nf, int T, int Tm,
+                                              float ambient_intensity, const float* ambient_color, float directional_intensity,
+                                              const float* directional_color, const float* direction, int with_specular, void* stream);
 
 B200R_API unsigned long long b200r_launch_count(void);
 

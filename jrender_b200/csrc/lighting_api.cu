@@ -12,7 +12,9 @@
 // The reference runs this as ~30 tensor ops over [B, nf, 3] intermediates (and as many again backward); in the
 // launch-bound demo loops that was ~230 launches per iteration.  Backward: the same expression re-evaluated in
 // forward-mode automatic differentiation over the 9 vertex coordinates (dual.cuh) -- the exact gradient of the
-// expression the forward evaluates, including the path through the normal, with 9 atomics per face into grad_vertices.
+// expression the forward evaluates, including the path through the normal, with 9 atomics per face into grad_vertices --
+// and, only when material gradients are requested, once more over the face's mean metallic and roughness (Dual<2>,
+// geometry constant), which keeps the vertex-only evaluation's code and registers as they were.
 #include "../../include/b200raster.h"
 #include "api_util.cuh"
 #include "dual.cuh"
@@ -27,9 +29,16 @@ struct LightParams {
     int with_specular;               // Cook-Torrance branch (needs eye + metallic + roughness)
 };
 
-template <class S> __device__ __forceinline__ S lift(float x);
-template <> __device__ __forceinline__ float lift<float>(float x) { return x; }
-template <> __device__ __forceinline__ Dual<9> lift<Dual<9>>(float x) { return dconst<9>(x); }
+// R: the result type of an expression mixing geometry of type S with material scalars of type M -- float when both are
+// float, Dual<N> when either is (face_light never mixes two Dual types).  lift<R>(x) widens a float or an R to an R.
+template <class S, class M> struct Promote { typedef S type; };
+template <int N> struct Promote<float, Dual<N>> { typedef Dual<N> type; };
+template <class R> struct Lift { __device__ __forceinline__ static R of(float x) { return x; } };
+template <int N> struct Lift<Dual<N>> {
+    __device__ __forceinline__ static Dual<N> of(float x) { return dconst<N>(x); }
+    __device__ __forceinline__ static Dual<N> of(const Dual<N>& x) { return x; }
+};
+template <class R, class X> __device__ __forceinline__ R lift(const X& x) { return Lift<R>::of(x); }
 
 template <class S>
 __device__ __forceinline__ S dot3(const S a[3], const S b[3]) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }   // torch.sum(a * b, dim): x, y, z order
@@ -44,37 +53,39 @@ __device__ __forceinline__ void normalize3(S x[3], float eps) {
     for (int k = 0; k < 3; k++) x[k] = x[k] / n;
 }
 
-// diffuse[3], specular[3] of one face from its normal N and centroid pos (directional_lighting.py:63-135, 3-D normals)
-template <class S>
-__device__ __forceinline__ void face_light(const S N[3], const S pos[3], const LightParams& L, const float* eye, float metallic,
-                                           float roughness, S diffuse[3], S specular[3]) {
+// diffuse[3], specular[3] of one face from its normal N and centroid pos (directional_lighting.py:63-135, 3-D normals).
+// S is the geometry's type and M the material scalars' (metallic, roughness): <float, float> evaluates, <Dual<9>, float>
+// differentiates w.r.t. the vertices, <float, Dual<2>> w.r.t. metallic and roughness with the geometry held constant.
+template <class S, class M, class R = typename Promote<S, M>::type>
+__device__ __forceinline__ void face_light(const S N[3], const S pos[3], const LightParams& L, const float* eye, M metallic,
+                                           M roughness, R diffuse[3], R specular[3]) {
     const S cosine = dmax(dot3f(N, L.dir), 0.f);   // relu(sum(normals * light_direction)) :66
 #pragma unroll
-    for (int c = 0; c < 3; c++) diffuse[c] = lift<S>(0.f + L.amb_i * L.amb_c[c]);   // zeros + ambient (ambient_lighting.py:8)
+    for (int c = 0; c < 3; c++) diffuse[c] = lift<R>(0.f + L.amb_i * L.amb_c[c]);   // zeros + ambient (ambient_lighting.py:8)
     if (L.with_specular && eye != nullptr) {
         S V[3] = {eye[0] - pos[0], eye[1] - pos[1], eye[2] - pos[2]};
         normalize3(V, 1e-12f);
         S H[3] = {V[0] + L.dir[0], V[1] + L.dir[1], V[2] + L.dir[2]};
         normalize3(H, 1e-12f);
-        const float a = roughness * roughness, a2 = a * a;
+        const M a = roughness * roughness, a2 = a * a;
         const S NdotH = dmax(dot3(N, H), 0.f);
-        S den = (NdotH * NdotH) * (a2 - 1.0f) + 1.0f;          // GGX :17
+        R den = (NdotH * NdotH) * (a2 - 1.0f) + 1.0f;          // GGX :17
         den = (den * 3.1415f) * den;                            // 3.1415 * denom * denom :18
-        const S NDF = lift<S>(a2) / den;
-        const float r1 = roughness + 1.0f, k = (r1 * r1) / 8.0f;
+        const R NDF = lift<R>(a2) / den;
+        const M r1 = roughness + 1.0f, k = (r1 * r1) / 8.0f;
         const S NdotV = dmax(dot3(N, V), 0.f), NdotL = dmax(dot3f(N, L.dir), 0.f);
-        const S G = (NdotL / (NdotL * (1.0f - k) + k)) * (NdotV / (NdotV * (1.0f - k) + k));   // GeometrySmith :34-46
+        const R G = (lift<R>(NdotL) / (NdotL * (1.0f - k) + k)) * (lift<R>(NdotV) / (NdotV * (1.0f - k) + k));   // GeometrySmith :34-46
         const S hv = 1.0f - dmax(dot3(H, V), 0.f);
         const S hv2 = hv * hv;
         const S p5 = (hv2 * hv2) * hv;                          // pow(1 - cosTheta, 5)
         S den4 = dmax((NdotV * 4.0f) * NdotL, 0.01f);          // clamp(4 N.V N.L, 0.01) :125-128
-        const S ndf_g = NDF * G;
+        const R ndf_g = NDF * G;
 #pragma unroll
         for (int c = 0; c < 3; c++) {
-            const float F0 = 0.4f * (1.f - metallic) + 1.0f * metallic;   // :103
-            const S Fr = F0 + (1.0f - F0) * p5;                           // fresnelSchlick :48-53
+            const M F0 = 0.4f * (1.f - metallic) + 1.0f * metallic;   // :103
+            const R Fr = F0 + (1.0f - F0) * p5;                           // fresnelSchlick :48-53
             const S radiance = (cosine * L.dir_c[c]) * L.dir_i;           // :105
-            const S KD = (1.0f - Fr) * (1.0f - metallic);                 // :117-119
+            const R KD = (1.0f - Fr) * (1.0f - metallic);                 // :117-119
             diffuse[c] = diffuse[c] + KD * radiance;
             specular[c] = ((ndf_g * Fr) / den4) * radiance;               // :122-129
         }
@@ -82,7 +93,7 @@ __device__ __forceinline__ void face_light(const S N[3], const S pos[3], const L
 #pragma unroll
         for (int c = 0; c < 3; c++) {
             diffuse[c] = diffuse[c] + (cosine * L.dir_c[c]) * L.dir_i;    // :131-135
-            specular[c] = lift<S>(0.f);
+            specular[c] = lift<R>(0.f);
         }
     }
 }
@@ -138,7 +149,8 @@ __global__ void __launch_bounds__(128)
 k_surface_lighting_bwd(const float* __restrict__ vertices, const int32_t* __restrict__ faces, const float* __restrict__ textures,
                        const float* __restrict__ metallic, const float* __restrict__ roughness, const float* __restrict__ eye,
                        const float* __restrict__ grad_out, float* __restrict__ grad_textures, float* __restrict__ grad_vertices,
-                       LightParams L, int B, int Bv, int Bf, int Be, int nv, int nf, int T, int Tm) {
+                       float* __restrict__ grad_metallic, float* __restrict__ grad_roughness, LightParams L, int B, int Bv, int Bf,
+                       int Be, int nv, int nf, int T, int Tm) {
     typedef Dual<9> D;
     const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= (long)B * nf) return;
@@ -179,6 +191,26 @@ k_surface_lighting_bwd(const float* __restrict__ vertices, const int32_t* __rest
             Gd[c] += g * x;
             Gs[c] += g;
         }
+    if (grad_metallic != nullptr || grad_roughness != nullptr) {
+        // derivatives of (diffuse, specular) w.r.t. the face's mean metallic and roughness, geometry held constant; each
+        // is spread evenly over the face's Tm texels (the gradient of the mean).  0 without the specular branch.
+        float gm = 0.f, gr = 0.f;
+        if (spec) {
+            Dual<2> dm[3], sm[3];
+            face_light<float, Dual<2>>(N, pos, Lf, ey, dvar<2>(m, 0), dvar<2>(r, 1), dm, sm);
+#pragma unroll
+            for (int c = 0; c < 3; c++) {
+                gm += Gd[c] * dm[c].d[0] + Gs[c] * sm[c].d[0];
+                gr += Gd[c] * dm[c].d[1] + Gs[c] * sm[c].d[1];
+            }
+            gm = gm / (float)Tm;
+            gr = gr / (float)Tm;
+        }
+        if (grad_metallic != nullptr)
+            for (int t = 0; t < Tm; t++) grad_metallic[(size_t)i * Tm + t] = gm;
+        if (grad_roughness != nullptr)
+            for (int t = 0; t < Tm; t++) grad_roughness[(size_t)i * Tm + t] = gr;
+    }
     if (grad_vertices == nullptr) return;
     // derivatives of (diffuse, specular) w.r.t. the 9 vertex coordinates
     D dv[9];
@@ -248,13 +280,16 @@ int b200r_surface_lighting_forward(const float* vertices, const int32_t* faces, 
 
 int b200r_surface_lighting_backward(const float* vertices, const int32_t* faces, const float* textures, const float* metallic,
                                     const float* roughness, const float* eye, const float* grad_out, float* grad_textures,
-                                    float* grad_vertices, int B, int vertices_batch, int faces_batch, int eye_batch, int nv, int nf,
-                                    int T, int Tm, float ambient_intensity, const float* ambient_color, float directional_intensity,
-                                    const float* directional_color, const float* direction, int with_specular, void* stream) {
+                                    float* grad_vertices, float* grad_metallic, float* grad_roughness, int B, int vertices_batch,
+                                    int faces_batch, int eye_batch, int nv, int nf, int T, int Tm, float ambient_intensity,
+                                    const float* ambient_color, float directional_intensity, const float* directional_color,
+                                    const float* direction, int with_specular, void* stream) {
     int rc = check_args("b200r_surface_lighting_backward", vertices, faces, textures, B, vertices_batch, faces_batch, eye_batch, nv, nf, T, Tm);
     if (rc) return rc;
     if (!grad_out || !grad_textures || !ambient_color || !directional_color || !direction)
         return b200r_fail(B200R_EINVAL, "b200r_surface_lighting_backward: NULL pointer argument");
+    if ((grad_metallic || grad_roughness) && (!metallic || !roughness || Tm == 0))
+        return b200r_fail(B200R_EINVAL, "b200r_surface_lighting_backward: material gradients need metallic, roughness and Tm > 0");
     cudaStream_t st = (cudaStream_t)stream;
     if (grad_vertices != nullptr) {
         cudaError_t e = cudaMemsetAsync(grad_vertices, 0, sizeof(float) * 3 * (size_t)vertices_batch * nv, st);
@@ -266,8 +301,9 @@ int b200r_surface_lighting_backward(const float* vertices, const int32_t* faces,
         B200rProfScope prof(B200R_K_LIGHTING, st);
         k_surface_lighting_bwd<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(vertices, faces, textures, metallic, roughness,
                                                                              eye_batch ? eye : nullptr, grad_out, grad_textures,
-                                                                             grad_vertices, L, B, vertices_batch, faces_batch,
-                                                                             eye_batch ? eye_batch : 1, nv, nf, T, Tm);
+                                                                             grad_vertices, grad_metallic, grad_roughness, L, B,
+                                                                             vertices_batch, faces_batch, eye_batch ? eye_batch : 1,
+                                                                             nv, nf, T, Tm);
     }
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return b200r_cuda_fail(e, "k_surface_lighting_bwd");

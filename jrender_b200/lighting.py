@@ -103,7 +103,8 @@ def directional_lighting(diffuseLight, specularLight, normals, light_intensity=0
 
 
 class _FusedSurfaceLighting(torch.autograd.Function):
-    """clamp(textures * diffuse + specular, 0, 1) with diffuse / specular from the face normals: b200r_surface_lighting_*."""
+    """clamp(textures * diffuse + specular, 0, 1) with diffuse / specular from the face normals: b200r_surface_lighting_*.
+    Differentiable w.r.t. vertices, textures, and metallic / roughness (through each face's mean material value)."""
 
     @staticmethod
     def forward(ctx, vertices, textures, faces, metallic, roughness, eye, params):
@@ -127,8 +128,10 @@ class _FusedSurfaceLighting(torch.autograd.Function):
         g = grad_out.contiguous()
         gt = torch.empty_like(tx)
         gv = torch.empty_like(v) if ctx.needs_input_grad[0] else None
-        _lib.call("b200r_surface_lighting_backward", v.device, v, faces, tx, metallic, roughness, eye, g, gt, gv, *ctx.args)
-        return gv, (gt if ctx.needs_input_grad[1] else None), None, None, None, None, None
+        gm = torch.empty_like(metallic) if ctx.needs_input_grad[3] else None
+        gr = torch.empty_like(roughness) if ctx.needs_input_grad[4] else None
+        _lib.call("b200r_surface_lighting_backward", v.device, v, faces, tx, metallic, roughness, eye, g, gt, gv, gm, gr, *ctx.args)
+        return gv, (gt if ctx.needs_input_grad[1] else None), None, gm, gr, None, None
 
 
 def _normalized_direction(d):
@@ -199,7 +202,7 @@ class Lighting(nn.Module):
             if n != 3:   # per-batch light colours / directions: op-by-op path
                 return False
         for t in (mesh.metallic_textures, mesh.roughness_textures):
-            if t is not None and (t.requires_grad or t.device != v.device or t.dtype != torch.float32
+            if t is not None and (t.device != v.device or t.dtype != torch.float32
                                   or t.shape[:2] != tx.shape[:2] or t.shape[-1] != 1):
                 return False
         if isinstance(eyes, torch.Tensor) and eyes.requires_grad:
