@@ -211,8 +211,6 @@ B200R_API int b200r_laplacian_loss(const float* vertices, const int32_t* neighbo
                                    const float* diag, float* loss, float* grad_vertices, int batch_size,
                                    int num_vertices, int max_degree, void* stream);
 
-/* Launch counter: number of kernels this library has launched in this process
- * (bench.py reports the delta over the timed region as "gpu_launches"). */
 /* ---- texture baking (SURVEY.md section 8f rank 3) -------------------------------------------------------------
  * Replaces _load_textures_for_softras / load_textures_cuda_kernel (jrender/io/utils/load_textures.py:3-101):
  * image [H, W, 3] f32 (already flipped vertically by the caller, _load_obj_for_softras.py:136), faces_uv [nf, 3, 2],
@@ -287,26 +285,29 @@ B200R_API int b200r_surface_lighting_backward(const float* vertices, const int32
                                               float ambient_intensity, const float* ambient_color, float directional_intensity,
                                               const float* directional_color, const float* direction, int with_specular, void* stream);
 
+/* Launch counter: number of kernels this library has launched in this process
+ * (bench.py reports the delta over the timed region as "gpu_launches"). */
 B200R_API unsigned long long b200r_launch_count(void);
 
-/* Tuning knobs (process-wide; results are identical for every setting except softras_exact_tail):
- *   "softras_fwd_persistent" 0 = one CTA per tile, 1 = persistent grid + tile queue (default)
+/* Tuning knobs (process-wide):
  *   "softras_exact_tail"     1 = the reference's double-precision sigmoid / alpha-product tails bit for bit;
  *                            0 (default) = the same expressions in fp32 for the default euclidean+softmax
  *                            mode (<= 1 ulp on D; all index / depth outputs are identical either way)
  *   "softras_list_pool_chunks" >= 0 caps the binning-list chunk pool (exercises the pool-exhausted path in tests);
- *                            -1 (default) = the size b200r_softras_workspace_bytes accounts for */
+ *                            -1 (default) = the size b200r_softras_workspace_bytes accounts for; results are
+ *                            identical for every setting */
 B200R_API int b200r_set_option(const char* name, int value);
 
 /* Per-kernel device timing (CUDA events recorded on the launch stream around every kernel
- * this library launches).  Off by default.  bench.py uses it for the roofline of the
- * dominant kernel; b200r_profile_read synchronises the outstanding events. */
+ * this library launches; each launch is counted under exactly one id).  Off by default.  bench.py
+ * uses it for the roofline of the dominant kernel; b200r_profile_read synchronises the outstanding
+ * events.  Ids are 0 .. B200R_K_COUNT - 1. */
 enum { B200R_K_FACE_SETUP = 0, B200R_K_COARSE_BIN = 1, B200R_K_SOFTRAS_FWD = 2, B200R_K_SOFTRAS_BWD = 3,
        B200R_K_TILE_ORDER = 4, B200R_K_NMR_SETUP = 5, B200R_K_NMR_FWD = 6, B200R_K_NMR_BWD_PIXEL = 7,
        B200R_K_NMR_BWD_MAPS = 8, B200R_K_SOFTRAS_BWD_FINALIZE = 9, B200R_K_NMR_PACK = 10,
        B200R_K_PROJECT_FWD = 11, B200R_K_PROJECT_BWD = 12, B200R_K_FLATTEN_LOSS = 13, B200R_K_LAPLACIAN_LOSS = 14,
        B200R_K_LIGHTING = 15, B200R_K_BAKE = 16, B200R_K_ATLAS = 17, B200R_K_VOXEL_SURFACE = 18,
-       B200R_K_VOXEL_FILL = 19 };
+       B200R_K_VOXEL_FILL = 19, B200R_K_CHUNK_RECTS = 20, B200R_K_DEBUG = 21, B200R_K_COUNT };
 B200R_API void b200r_profile_enable(int on);
 B200R_API void b200r_profile_reset(void);
 B200R_API int b200r_profile_read(int kernel, double* total_ms, long long* launches);

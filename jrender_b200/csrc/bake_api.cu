@@ -130,25 +130,13 @@ extern "C" int b200r_bake_textures_n3mr(const float* image, const float* faces_u
     if (texture_wrapping < 0 || texture_wrapping > 3) return b200r_fail(B200R_EINVAL, "b200r_bake_textures_n3mr: texture_wrapping %d outside [0, 3]", texture_wrapping);
     cudaStream_t st = (cudaStream_t)stream;
     const long ntexels = (long)nf * texture_size * texture_size * texture_size;
-    const unsigned grid = (unsigned)((ntexels + 255) / 256);
-    {
-        B200rProfScope prof(B200R_K_BAKE, st);
-#define B200R_BAKE_N3MR(WR, BL) k_bake_textures_n3mr<WR, BL><<<grid, 256, 0, st>>>(image, faces_uv, is_update, textures, ntexels, texture_size, image_height, image_width)
-        switch (texture_wrapping * 2 + (use_bilinear ? 1 : 0)) {
-            case 0: B200R_BAKE_N3MR(0, false); break;
-            case 1: B200R_BAKE_N3MR(0, true); break;
-            case 2: B200R_BAKE_N3MR(1, false); break;
-            case 3: B200R_BAKE_N3MR(1, true); break;
-            case 4: B200R_BAKE_N3MR(2, false); break;
-            case 5: B200R_BAKE_N3MR(2, true); break;
-            case 6: B200R_BAKE_N3MR(3, false); break;
-            default: B200R_BAKE_N3MR(3, true); break;
-        }
-#undef B200R_BAKE_N3MR
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_bake_textures_n3mr");
-    return 0;
+    // indexed by texture_wrapping * 2 + use_bilinear
+    static constexpr decltype(&k_bake_textures_n3mr<0, false>) kernels[8] = {
+        k_bake_textures_n3mr<0, false>, k_bake_textures_n3mr<0, true>, k_bake_textures_n3mr<1, false>, k_bake_textures_n3mr<1, true>,
+        k_bake_textures_n3mr<2, false>, k_bake_textures_n3mr<2, true>, k_bake_textures_n3mr<3, false>, k_bake_textures_n3mr<3, true>};
+    return b200r_launch("k_bake_textures_n3mr", B200R_K_BAKE, kernels[texture_wrapping * 2 + (use_bilinear ? 1 : 0)],
+                        (unsigned)((ntexels + 255) / 256), 256, 0, st, image, faces_uv, is_update, textures, ntexels, texture_size,
+                        image_height, image_width);
 }
 
 extern "C" int b200r_bake_textures_softras(const float* image, const float* faces_uv, const int32_t* is_update, float* textures,
@@ -158,12 +146,6 @@ extern "C" int b200r_bake_textures_softras(const float* image, const float* face
         return b200r_fail(B200R_EINVAL, "b200r_bake_textures_softras: non-positive size");
     cudaStream_t st = (cudaStream_t)stream;
     const long ntexels = (long)nf * texture_res * texture_res;
-    {
-        B200rProfScope prof(B200R_K_BAKE, st);
-        k_bake_textures_softras<<<(unsigned)((ntexels + 255) / 256), 256, 0, st>>>(image, faces_uv, is_update, textures, ntexels, texture_res,
-                                                                                  image_height, image_width);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_bake_textures_softras");
-    return 0;
+    return b200r_launch("k_bake_textures_softras", B200R_K_BAKE, k_bake_textures_softras, (unsigned)((ntexels + 255) / 256), 256, 0, st,
+                        image, faces_uv, is_update, textures, ntexels, texture_res, image_height, image_width);
 }

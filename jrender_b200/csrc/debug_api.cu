@@ -62,8 +62,6 @@ __global__ void k_debug_exact_math(const float* __restrict__ a, const float* __r
 extern "C" B200R_API int b200r_debug_exact_math(const float* a, const float* b, int n, int* mismatch7, void* stream) {
     if (!a || !b || !mismatch7 || n <= 0) return b200r_fail(B200R_EINVAL, "b200r_debug_exact_math: bad argument");
     cudaStream_t st = (cudaStream_t)stream;
-    cudaMemsetAsync(mismatch7, 0, 7 * sizeof(int), st);
-    k_debug_exact_math<<<(n + 255) / 256, 256, 0, st>>>(a, b, n, mismatch7);
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : b200r_cuda_fail(e, "k_debug_exact_math");
+    if (int rc = b200r_zero(mismatch7, 7 * sizeof(int), st, "memset mismatch counts")) return rc;
+    return b200r_launch("k_debug_exact_math", B200R_K_DEBUG, k_debug_exact_math, (n + 255) / 256, 256, 0, st, a, b, n, mismatch7);
 }

@@ -267,15 +267,9 @@ int b200r_surface_lighting_forward(const float* vertices, const int32_t* faces, 
     cudaStream_t st = (cudaStream_t)stream;
     const LightParams L = make(ambient_intensity, ambient_color, directional_intensity, directional_color, direction, with_specular);
     const long total = (long)B * nf;
-    {
-        B200rProfScope prof(B200R_K_LIGHTING, st);
-        k_surface_lighting_fwd<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(vertices, faces, textures, metallic, roughness,
-                                                                             eye_batch ? eye : nullptr, out_textures, L, B, vertices_batch,
-                                                                             faces_batch, eye_batch ? eye_batch : 1, nv, nf, T, Tm);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_surface_lighting_fwd");
-    return 0;
+    return b200r_launch("k_surface_lighting_fwd", B200R_K_LIGHTING, k_surface_lighting_fwd, (unsigned)((total + 127) / 128), 128, 0, st,
+                        vertices, faces, textures, metallic, roughness, eye_batch ? eye : nullptr, out_textures, L, B,
+                        vertices_batch, faces_batch, eye_batch ? eye_batch : 1, nv, nf, T, Tm);
 }
 
 int b200r_surface_lighting_backward(const float* vertices, const int32_t* faces, const float* textures, const float* metallic,
@@ -292,22 +286,14 @@ int b200r_surface_lighting_backward(const float* vertices, const int32_t* faces,
         return b200r_fail(B200R_EINVAL, "b200r_surface_lighting_backward: material gradients need metallic, roughness and Tm > 0");
     cudaStream_t st = (cudaStream_t)stream;
     if (grad_vertices != nullptr) {
-        cudaError_t e = cudaMemsetAsync(grad_vertices, 0, sizeof(float) * 3 * (size_t)vertices_batch * nv, st);
-        if (e != cudaSuccess) return b200r_cuda_fail(e, "memset grad_vertices");
+        if (int rc = b200r_zero(grad_vertices, sizeof(float) * 3 * (size_t)vertices_batch * nv, st, "memset grad_vertices")) return rc;
     }
     const LightParams L = make(ambient_intensity, ambient_color, directional_intensity, directional_color, direction, with_specular);
     const long total = (long)B * nf;
-    {
-        B200rProfScope prof(B200R_K_LIGHTING, st);
-        k_surface_lighting_bwd<<<(unsigned)((total + 127) / 128), 128, 0, st>>>(vertices, faces, textures, metallic, roughness,
-                                                                             eye_batch ? eye : nullptr, grad_out, grad_textures,
-                                                                             grad_vertices, grad_metallic, grad_roughness, L, B,
-                                                                             vertices_batch, faces_batch, eye_batch ? eye_batch : 1,
-                                                                             nv, nf, T, Tm);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_surface_lighting_bwd");
-    return 0;
+    return b200r_launch("k_surface_lighting_bwd", B200R_K_LIGHTING, k_surface_lighting_bwd, (unsigned)((total + 127) / 128), 128, 0, st,
+                        vertices, faces, textures, metallic, roughness, eye_batch ? eye : nullptr, grad_out, grad_textures,
+                        grad_vertices, grad_metallic, grad_roughness, L, B, vertices_batch, faces_batch,
+                        eye_batch ? eye_batch : 1, nv, nf, T, Tm);
 }
 
 }  // extern "C"

@@ -171,9 +171,8 @@ k_laplacian_loss(const float* __restrict__ vertices, const int32_t* __restrict__
 }
 
 int zero_outputs(const char* who, float* loss, float* grad, int B, int nv, cudaStream_t st) {
-    cudaError_t e = cudaMemsetAsync(loss, 0, sizeof(float) * (size_t)B, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(grad, 0, sizeof(float) * 3 * (size_t)B * nv, st);
-    return e == cudaSuccess ? 0 : b200r_cuda_fail(e, who);
+    if (int rc = b200r_zero(loss, sizeof(float) * (size_t)B, st, who)) return rc;
+    return b200r_zero(grad, sizeof(float) * 3 * (size_t)B * nv, st, who);
 }
 
 }  // namespace
@@ -190,13 +189,8 @@ B200R_API int b200r_flatten_loss(const float* vertices, const int32_t* v0s, cons
     cudaStream_t st = (cudaStream_t)stream;
     int rc = zero_outputs("b200r_flatten_loss: memset", loss, grad_vertices, batch_size, num_vertices, st);
     if (rc || num_edges == 0) return rc;
-    {
-        B200rProfScope scope(B200R_K_FLATTEN_LOSS, st);
-        k_flatten_loss<<<dim3((num_edges + 127) / 128, batch_size), 128, 0, st>>>(vertices, v0s, v1s, v2s, v3s, loss, grad_vertices,
-                                                                                  num_vertices, num_edges, eps);
-    }
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : b200r_cuda_fail(e, "k_flatten_loss");
+    return b200r_launch("k_flatten_loss", B200R_K_FLATTEN_LOSS, k_flatten_loss, dim3((num_edges + 127) / 128, batch_size), 128, 0, st,
+                        vertices, v0s, v1s, v2s, v3s, loss, grad_vertices, num_vertices, num_edges, eps);
 }
 
 B200R_API int b200r_laplacian_loss(const float* vertices, const int32_t* neighbours, const float* neighbour_weights,
@@ -209,13 +203,8 @@ B200R_API int b200r_laplacian_loss(const float* vertices, const int32_t* neighbo
     cudaStream_t st = (cudaStream_t)stream;
     int rc = zero_outputs("b200r_laplacian_loss: memset", loss, grad_vertices, batch_size, num_vertices, st);
     if (rc) return rc;
-    {
-        B200rProfScope scope(B200R_K_LAPLACIAN_LOSS, st);
-        k_laplacian_loss<<<dim3((num_vertices + 127) / 128, batch_size), 128, 0, st>>>(vertices, neighbours, neighbour_weights, diag,
-                                                                                       loss, grad_vertices, num_vertices, max_degree);
-    }
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : b200r_cuda_fail(e, "k_laplacian_loss");
+    return b200r_launch("k_laplacian_loss", B200R_K_LAPLACIAN_LOSS, k_laplacian_loss, dim3((num_vertices + 127) / 128, batch_size), 128,
+                        0, st, vertices, neighbours, neighbour_weights, diag, loss, grad_vertices, num_vertices, max_degree);
 }
 
 }  // extern "C"

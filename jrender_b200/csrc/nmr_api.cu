@@ -41,22 +41,13 @@ int b200r_nmr_forward(const float* faces, const float* textures, int32_t* face_i
     cudaError_t e = cudaMemsetAsync(zbuf, 0xFF, need, st);   // every pixel: "no face yet"
     if (e != cudaSuccess) return b200r_cuda_fail(e, "memset z-buffer");
     const long nfaces = (long)B * nf;
-    {
-        B200rProfScope prof(B200R_K_NMR_SETUP, st);
-        k_nmr_zbuffer<<<(unsigned)((nfaces + 255) / 256), 256, 0, st>>>(faces, zbuf, B, nf, is, near_, far_);
-    }
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_nmr_zbuffer");
+    if (int rc = b200r_launch("k_nmr_zbuffer", B200R_K_NMR_SETUP, k_nmr_zbuffer, (unsigned)((nfaces + 255) / 256), 256, 0, st,
+                              faces, zbuf, B, nf, is, near_, far_))
+        return rc;
     const size_t npix = (size_t)B * is * is;
-    {
-        B200rProfScope prof(B200R_K_NMR_FWD, st);
-        k_nmr_resolve<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(P, zbuf, faces, textures, face_index_map, weight_map, depth_map,
-                                                                     rgb_map, alpha_map, sampling_index_map, sampling_weight_map,
-                                                                     face_inv_map);
-    }
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_nmr_resolve");
-    return 0;
+    return b200r_launch("k_nmr_resolve", B200R_K_NMR_FWD, k_nmr_resolve, (unsigned)((npix + 255) / 256), 256, 0, st, P, zbuf, faces,
+                        textures, face_index_map, weight_map, depth_map, rgb_map, alpha_map, sampling_index_map,
+                        sampling_weight_map, face_inv_map);
 }
 
 size_t b200r_nmr_backward_scratch_bytes(int batch_size, int image_size) {
@@ -79,11 +70,10 @@ int b200r_nmr_backward(const float* faces, const int32_t* face_index_map, const 
     if (return_depth && (!depth_map || !weight_map || !face_inv_map || !grad_depth_map))
         return b200r_fail(B200R_EINVAL, "b200r_nmr_backward: return_depth needs depth_map, weight_map, face_inv_map, grad_depth_map");
     cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = cudaMemsetAsync(grad_faces, 0, sizeof(float) * 9 * (size_t)B * nf, st);   // rasterize.py:623
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "memset grad_faces");
+    if (int rc = b200r_zero(grad_faces, sizeof(float) * 9 * (size_t)B * nf, st, "memset grad_faces")) return rc;   // rasterize.py:623
     if (return_rgb) {
-        e = cudaMemsetAsync(grad_textures, 0, sizeof(float) * 3 * (size_t)texture_size * texture_size * texture_size * B * nf, st);  // :705
-        if (e != cudaSuccess) return b200r_cuda_fail(e, "memset grad_textures");
+        const size_t bytes = sizeof(float) * 3 * (size_t)texture_size * texture_size * texture_size * B * nf;
+        if (int rc = b200r_zero(grad_textures, bytes, st, "memset grad_textures")) return rc;   // :705
     }
     if (return_rgb || return_alpha) {  // n3mr.py:150-154
         const size_t need = b200r_nmr_backward_scratch_bytes(B, is);
@@ -94,37 +84,21 @@ int b200r_nmr_backward(const float* faces, const int32_t* face_index_map, const 
         float* ph = reinterpret_cast<float*>(scratch);
         float* pv = ph + (size_t)B * is * is * fl;
         const long warps = (long)B * nf;
-#define B200R_LAUNCH_K9(MODE)                                                                                                          \
-    {                                                                                                                                  \
-        {                                                                                                                              \
-            B200rProfScope prof(B200R_K_NMR_PACK, st);                                                                                 \
-            k_nmr_pack<MODE><<<dim3((is + 31) / 32, (is + 31) / 32, B), 256, 0, st>>>(rgb_map, alpha_map, grad_rgb_map, grad_alpha_map, \
-                                                                                    ph, pv, is);                                      \
-        }                                                                                                                              \
-        e = cudaGetLastError();                                                                                                        \
-        if (e != cudaSuccess) return b200r_cuda_fail(e, "k_nmr_pack");                                                                 \
-        B200rProfScope prof(B200R_K_NMR_BWD_PIXEL, st);                                                                                \
-        k_nmr_backward_pixel_map<MODE><<<(unsigned)((warps + 7) / 8), 256, 0, st>>>(faces, face_index_map, rgb_map, alpha_map, ph, pv,  \
-                                                                                   grad_faces, B, nf, is, eps);                       \
+        auto pack = mode == 3 ? &k_nmr_pack<3> : mode == 1 ? &k_nmr_pack<1> : &k_nmr_pack<2>;
+        auto pixel_map = mode == 3 ? &k_nmr_backward_pixel_map<3> : mode == 1 ? &k_nmr_backward_pixel_map<1> : &k_nmr_backward_pixel_map<2>;
+        if (int rc = b200r_launch("k_nmr_pack", B200R_K_NMR_PACK, pack, dim3((is + 31) / 32, (is + 31) / 32, B), 256, 0, st, rgb_map,
+                                  alpha_map, grad_rgb_map, grad_alpha_map, ph, pv, is))
+            return rc;
+        if (int rc = b200r_launch("k_nmr_backward_pixel_map", B200R_K_NMR_BWD_PIXEL, pixel_map, (unsigned)((warps + 7) / 8), 256, 0,
+                                  st, faces, face_index_map, rgb_map, alpha_map, ph, pv, grad_faces, B, nf, is, eps))
+            return rc;
     }
-        if (mode == 3) B200R_LAUNCH_K9(3)
-        else if (mode == 1) B200R_LAUNCH_K9(1)
-        else B200R_LAUNCH_K9(2)
-#undef B200R_LAUNCH_K9
-    }
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_nmr_backward_pixel_map");
-    if (return_rgb || return_depth) {
-        const size_t npix = (size_t)B * is * is;
-        B200rProfScope prof(B200R_K_NMR_BWD_MAPS, st);
-        k_nmr_backward_maps<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(faces, face_index_map, weight_map, depth_map, face_inv_map,
-                                                                           sampling_index_map, sampling_weight_map, grad_rgb_map,
-                                                                           grad_depth_map, grad_faces, grad_textures, B, nf, is,
-                                                                           texture_size, return_rgb ? 1 : 0, return_depth ? 1 : 0);
-    }
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_nmr_backward_maps");
-    return 0;
+    if (!return_rgb && !return_depth) return 0;
+    const size_t npix = (size_t)B * is * is;
+    return b200r_launch("k_nmr_backward_maps", B200R_K_NMR_BWD_MAPS, k_nmr_backward_maps, (unsigned)((npix + 255) / 256), 256, 0, st,
+                        faces, face_index_map, weight_map, depth_map, face_inv_map, sampling_index_map, sampling_weight_map,
+                        grad_rgb_map, grad_depth_map, grad_faces, grad_textures, B, nf, is, texture_size, return_rgb ? 1 : 0,
+                        return_depth ? 1 : 0);
 }
 
 }  // extern "C"

@@ -103,7 +103,7 @@ k_project_faces_fwd(const CamParams C, const float* __restrict__ vertices, const
 
 // Backward: d(loss)/d(world vertex) accumulated over every (face, corner) that references the
 // vertex (and over the batch when the vertices are shared).  grad_vertices is zeroed by the caller
-// of the kernel (cudaMemsetAsync in the entry point).
+// of the kernel (b200r_zero in the entry point).
 __global__ void __launch_bounds__(256)
 k_project_faces_bwd(const CamParams C, const float* __restrict__ vertices, const int32_t* __restrict__ faces,
                     const float* __restrict__ eyes, const float* __restrict__ grad_face_vertices,
@@ -179,12 +179,8 @@ B200R_API int b200r_project_faces_forward(const float* vertices, const int32_t* 
     const CamParams C = make_params(at_or_direction, up, width_or_scale, camera_mode, projection, batch_size, num_vertices,
                                     num_faces, vertices_batch, faces_batch, eye_batch);
     const long long n = (long long)batch_size * num_faces * 3;
-    {
-        B200rProfScope scope(B200R_K_PROJECT_FWD, st);
-        k_project_faces_fwd<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(C, vertices, faces, eye, face_vertices);
-    }
-    cudaError_t e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : b200r_cuda_fail(e, "k_project_faces_fwd");
+    return b200r_launch("k_project_faces_fwd", B200R_K_PROJECT_FWD, k_project_faces_fwd, (unsigned)((n + 255) / 256), 256, 0, st, C,
+                        vertices, faces, eye, face_vertices);
 }
 
 B200R_API int b200r_project_faces_backward(const float* vertices, const int32_t* faces, const float* eye,
@@ -200,14 +196,11 @@ B200R_API int b200r_project_faces_backward(const float* vertices, const int32_t*
     const CamParams C = make_params(at_or_direction, up, width_or_scale, camera_mode, projection, batch_size, num_vertices,
                                     num_faces, vertices_batch, faces_batch, eye_batch);
     const long long n = (long long)batch_size * num_faces * 3;
-    cudaError_t e = cudaMemsetAsync(grad_vertices, 0, sizeof(float) * 3 * (size_t)vertices_batch * num_vertices, st);
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "b200r_project_faces_backward: memset");
-    {
-        B200rProfScope scope(B200R_K_PROJECT_BWD, st);
-        k_project_faces_bwd<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(C, vertices, faces, eye, grad_face_vertices, grad_vertices);
-    }
-    e = cudaGetLastError();
-    return e == cudaSuccess ? 0 : b200r_cuda_fail(e, "k_project_faces_bwd");
+    if (int rc = b200r_zero(grad_vertices, sizeof(float) * 3 * (size_t)vertices_batch * num_vertices, st,
+                            "b200r_project_faces_backward: memset"))
+        return rc;
+    return b200r_launch("k_project_faces_bwd", B200R_K_PROJECT_BWD, k_project_faces_bwd, (unsigned)((n + 255) / 256), 256, 0, st, C,
+                        vertices, faces, eye, grad_face_vertices, grad_vertices);
 }
 
 }  // extern "C"

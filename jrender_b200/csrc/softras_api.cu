@@ -13,7 +13,6 @@ using namespace b200r;
 
 namespace {
 
-std::atomic<int> g_fwd_persistent{1};  // 0: one CTA per tile, 1: persistent grid + atomic tile queue
 std::atomic<int> g_exact_tail{0};      // 1: reference's double-precision sigmoid / alpha tails bit for bit; 0: fp32 tails (<= 1 ulp)
 std::atomic<int> g_pool_cap{-1};       // >= 0: cap on the coarse-list chunk pool (tests of the pool-exhausted path); -1: the carved size
 }  // namespace
@@ -59,7 +58,6 @@ const char* b200r_version(void) { return "b200raster 0.1 (sm_90a)"; }
 
 int b200r_set_option(const char* name, int value) {
     if (!name) return b200r_fail(B200R_EINVAL, "b200r_set_option: NULL name");
-    if (!strcmp(name, "softras_fwd_persistent")) { g_fwd_persistent.store(value ? 1 : 0); return 0; }
     if (!strcmp(name, "softras_exact_tail")) { g_exact_tail.store(value ? 1 : 0); return 0; }
     if (!strcmp(name, "softras_list_pool_chunks")) { g_pool_cap.store(value < 0 ? -1 : value); return 0; }
     return b200r_fail(B200R_EINVAL, "b200r_set_option: unknown option '%s'", name);
@@ -99,39 +97,22 @@ static int softras_forward_impl(const float* face_vertices, const float* texture
     const float border = sqrtf(dist_eps_logit * sigma_val);  // sqrt(threshold), :289,:316 (IEEE sqrt on host == device)
 
     const int total = B * nf;
-    {
-        B200rProfScope prof(B200R_K_FACE_SETUP, st);
-        k_face_setup<<<(total + 255) / 256, 256, 0, st>>>(face_vertices, textures, W.recs, W.rects, faces_info, total, nf, T, texture_type, is, border);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_face_setup");
-
-    e = cudaMemsetAsync(W.counters, 0, 256 * sizeof(int), st);
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "memset counters");
-    {
-        B200rProfScope prof(B200R_K_COARSE_BIN, st);
-        k_chunk_rects<<<dim3((nf + 255) / 256, B), 256, 0, st>>>(W.rects, W.chunk_rects, nf);
-        k_coarse_bin<<<dim3(P.ncs * P.ncs, B), 256, 0, st>>>(W.rects, W.chunk_rects, W.coarse_cnt, W.chunk_table, W.coarse_pool, W.counters + 1,
-                                                             W.chunks_per_bin, W.pool_chunks, W.tile_cost, W.counters + 64,
-                                                             nf, is, P.coarse_px, P.ncs, P.fntx, P.fnty);
-    }
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_coarse_bin");
+    if (int rc = b200r_launch("k_face_setup", B200R_K_FACE_SETUP, k_face_setup, (total + 255) / 256, 256, 0, st, face_vertices,
+                              textures, W.recs, W.rects, faces_info, total, nf, T, texture_type, is, border))
+        return rc;
+    if (int rc = b200r_zero(W.counters, 256 * sizeof(int), st, "memset counters")) return rc;
+    if (int rc = b200r_launch("k_chunk_rects", B200R_K_CHUNK_RECTS, k_chunk_rects, dim3((nf + 255) / 256, B), 256, 0, st, W.rects,
+                              W.chunk_rects, nf))
+        return rc;
+    if (int rc = b200r_launch("k_coarse_bin", B200R_K_COARSE_BIN, k_coarse_bin, dim3(P.ncs * P.ncs, B), 256, 0, st, W.rects,
+                              W.chunk_rects, W.coarse_cnt, W.chunk_table, W.coarse_pool, W.counters + 1, W.chunks_per_bin,
+                              W.pool_chunks, W.tile_cost, W.counters + 64, nf, is, P.coarse_px, P.ncs, P.fntx, P.fnty))
+        return rc;
     // k_tile_order writes a permutation of all queue_len slots: no holes to pre-fill
-    {
-        B200rProfScope prof(B200R_K_TILE_ORDER, st);
-        k_tile_order<<<(P.queue_len + 255) / 256, 256, 0, st>>>(W.tile_cost, W.counters + 64, W.counters + 128, W.tile_order,
-                                                                B, P.fntx, P.fnty);
-    }
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_tile_order");
-
-    {
-        const int persistent = g_fwd_persistent.load(), exact = g_exact_tail.load();
-        e = b200r_launch_forward(P, W, textures, soft_colors, aggrs_info, faces_id_buffer, pooled, persistent, exact, st);
-    }
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_softras_forward");
-    return 0;
+    if (int rc = b200r_launch("k_tile_order", B200R_K_TILE_ORDER, k_tile_order, (P.queue_len + 255) / 256, 256, 0, st,
+                              W.tile_cost, W.counters + 64, W.counters + 128, W.tile_order, B, P.fntx, P.fnty))
+        return rc;
+    return b200r_launch_forward(P, W, textures, soft_colors, aggrs_info, faces_id_buffer, pooled, g_exact_tail.load(), st);
 }
 
 int b200r_softras_forward(const float* face_vertices, const float* textures, float* soft_colors,
@@ -173,11 +154,8 @@ static int softras_backward_impl(const float* face_vertices, const float* textur
     SoftRasParams P = make_params(B, nf, T, is, K, near_, far_, eps, sigma_val, gamma_val, dist_eps_logit,
                                   dist_func, rgb_func, alpha_func, texture_type, double_side);
     P.aa = grad_is_pooled ? 1 : 0;
-    cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = b200r_launch_backward(P, W, textures, soft_colors, aggrs_info, faces_id_buffer, grad_soft_colors,
-                                          grad_face_vertices, grad_textures, g_exact_tail.load(), st);
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_softras_backward");
-    return 0;
+    return b200r_launch_backward(P, W, textures, soft_colors, aggrs_info, faces_id_buffer, grad_soft_colors, grad_face_vertices,
+                                 grad_textures, g_exact_tail.load(), (cudaStream_t)stream);
 }
 
 int b200r_softras_backward(const float* face_vertices, const float* textures, const float* soft_colors,

@@ -11,9 +11,9 @@
 // id): each pixel visits its faces in ascending id exactly like the reference's `for (fn = 0; fn < nf; fn++)` (:311),
 // minus the faces check_border would skip.
 //
-// Scheduling: `tile_counter == nullptr` -> one CTA per block (blockIdx); otherwise a persistent grid pulls blocks from an
-// atomic queue ordered by descending cost (number of (pixel, face) pairs per block, computed by k_coarse_bin and
-// bucket-sorted by k_tile_order): blocks at poles / silhouettes of a mesh can cost 10x the mean and must start first.
+// Scheduling: a persistent grid pulls blocks from an atomic queue (head `tile_counter`) ordered by descending cost
+// (number of (pixel, face) pairs per block, computed by k_coarse_bin and bucket-sorted by k_tile_order): blocks at
+// poles / silhouettes of a mesh can cost 10x the mean and must start first.
 #pragma once
 #include "softras_math.cuh"
 #include "softras_setup.cuh"
@@ -34,7 +34,7 @@ static_assert(B200R_BLOCK_W * B200R_BLOCK_H == kFwdLanes, "one lane per pixel of
 
 // resident one-warp CTAs per SM the register allocation must allow (96 registers).  H100, C3: forward 1.08 ms at 20, 1.10
 // at 16, 1.29 at 24 (16-record rounds, LDG staging); with bulk copies 1.017 at 20, 1.016 at 22, 1.017 at 18.  Spills
-// (ptxas, sm_90a): the C3 instantiation <2,1,false> 72 B stored / 80 B loaded at 96 registers; the others 0-52 B
+// (ptxas, sm_90a): the C3 instantiation <2,1,false> 64 B stored / 72 B loaded at 96 registers; the others 0-8 B
 constexpr int kFwdMinBlocks = 20;
 
 // ---- mbarrier / bulk-copy (TMA) helpers.  Records are staged by cp.async.bulk + mbarrier rather than LDG -> registers
@@ -363,27 +363,18 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
     __syncwarp();
     uint32_t parity = 0;
 
-    for (int titer = 0;; titer++) {
+    for (;;) {
         // ---- which block
-        int b, tx, ty;
-        bool empty = false;   // no face rectangle touches the block (k_coarse_bin's exact per-block count is 0)
-        if (tile_counter == nullptr) {
-            if (titer > 0) break;
-            b = blockIdx.y;
-            tx = blockIdx.x % P.fntx;
-            ty = blockIdx.x / P.fntx;
-        } else {
-            __syncwarp();  // previous block fully written
-            int q = 0;
-            if (lane == 0) q = atomicAdd(tile_counter, 1);
-            q = __shfl_sync(FULL, q, 0);
-            if (q >= P.queue_len) break;
-            const uint2 te = __ldg(tile_order + q);  // most expensive blocks first (k_tile_order): x | y << 16, image | empty << 31
-            tx = (int)(te.x & 0xffffu);
-            ty = (int)(te.x >> 16);
-            b = (int)(te.y & 0x7fffffffu);
-            empty = (te.y >> 31) != 0u;
-        }
+        __syncwarp();  // previous block fully written
+        int q = 0;
+        if (lane == 0) q = atomicAdd(tile_counter, 1);
+        q = __shfl_sync(FULL, q, 0);
+        if (q >= P.queue_len) break;
+        const uint2 te = __ldg(tile_order + q);  // most expensive blocks first (k_tile_order): x | y << 16, image | empty << 31
+        const int tx = (int)(te.x & 0xffffu);
+        const int ty = (int)(te.x >> 16);
+        const int b = (int)(te.y & 0x7fffffffu);
+        const bool empty = (te.y >> 31) != 0u;   // no face rectangle touches the block (k_coarse_bin's exact per-block count is 0)
         const int tx0 = tx * TW, tr0 = ty * TH;   // block origin
         const int px = tx0 + lx, row = tr0 + ly;
 

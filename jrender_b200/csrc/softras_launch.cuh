@@ -6,13 +6,14 @@
 
 #include "common.cuh"
 
+// Both return 0 or a failure already recorded for b200r_last_error.
 // pooled: optional [B,4,is/2,is/2] 2x2 mean of soft_colors written by the forward (anti-aliasing epilogue), or nullptr
-cudaError_t b200r_launch_forward(const SoftRasParams& P, const SoftRasWorkspace& W, const float* textures, float* soft_colors,
-                                 float* aggrs_info, int32_t* ids, float* pooled, int persistent, int exact, cudaStream_t st);
-cudaError_t b200r_launch_backward(const SoftRasParams& P, const SoftRasWorkspace& W, const float* textures,
-                                  const float* soft_colors, const float* aggrs_info, const int32_t* ids,
-                                  const float* grad_soft_colors, float* grad_faces, float* grad_textures,
-                                  int exact, cudaStream_t st);
+int b200r_launch_forward(const SoftRasParams& P, const SoftRasWorkspace& W, const float* textures, float* soft_colors,
+                         float* aggrs_info, int32_t* ids, float* pooled, int exact, cudaStream_t st);
+int b200r_launch_backward(const SoftRasParams& P, const SoftRasWorkspace& W, const float* textures,
+                          const float* soft_colors, const float* aggrs_info, const int32_t* ids,
+                          const float* grad_soft_colors, float* grad_faces, float* grad_textures,
+                          int exact, cudaStream_t st);
 
 // runs the statement(s) with D = P.dist_func and R = P.rgb_func as compile-time constants
 #define B200R_DISPATCH_DIST_RGB(...)                                       \

@@ -145,14 +145,8 @@ extern "C" int b200r_texture_atlas_softras(const float* tile_vertices, const flo
     if (texture_res < 1) return b200r_fail(B200R_EINVAL, "b200r_texture_atlas_softras: texture_res %d < 1", texture_res);
     cudaStream_t st = (cudaStream_t)stream;
     const long npix = (long)image_height * image_width;
-    {
-        B200rProfScope prof(B200R_K_ATLAS, st);
-        k_texture_atlas_softras<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(tile_vertices, textures, image, nf, texture_res,
-                                                                              texture_res_out, tile_width, npix, image_width);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_texture_atlas_softras");
-    return 0;
+    return b200r_launch("k_texture_atlas_softras", B200R_K_ATLAS, k_texture_atlas_softras, (unsigned)((npix + 255) / 256), 256, 0, st,
+                        tile_vertices, textures, image, nf, texture_res, texture_res_out, tile_width, npix, image_width);
 }
 
 extern "C" int b200r_texture_atlas_n3mr(const float* tile_vertices, const float* textures, float* image, int nf,
@@ -165,12 +159,6 @@ extern "C" int b200r_texture_atlas_n3mr(const float* tile_vertices, const float*
         return b200r_fail(B200R_EINVAL, "b200r_texture_atlas_n3mr: texture_size %d < 2", texture_size);
     cudaStream_t st = (cudaStream_t)stream;
     const long npix = (long)image_height * image_width;
-    {
-        B200rProfScope prof(B200R_K_ATLAS, st);
-        k_texture_atlas_n3mr<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>(tile_vertices, textures, image, nf, texture_size,
-                                                                           texture_res_out, tile_width, npix, image_width);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_texture_atlas_n3mr");
-    return 0;
+    return b200r_launch("k_texture_atlas_n3mr", B200R_K_ATLAS, k_texture_atlas_n3mr, (unsigned)((npix + 255) / 256), 256, 0, st,
+                        tile_vertices, textures, image, nf, texture_size, texture_res_out, tile_width, npix, image_width);
 }

@@ -274,16 +274,10 @@ extern "C" int b200r_voxelize_surface(const float* faces, int32_t* voxels, int b
     if (num_faces < 1) return b200r_fail(B200R_EINVAL, "b200r_voxelize_surface: num_faces %d < 1", num_faces);
     cudaStream_t st = (cudaStream_t)stream;
     const size_t vs3 = (size_t)voxel_size * voxel_size * voxel_size;
-    cudaError_t e = cudaMemsetAsync(voxels, 0, (size_t)batch_size * vs3 * sizeof(int32_t), st);
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "b200r_voxelize_surface: memset");
+    if (int rc = b200r_zero(voxels, (size_t)batch_size * vs3 * sizeof(int32_t), st, "b200r_voxelize_surface: memset")) return rc;
     const long total = (long)batch_size * num_faces;
-    {
-        B200rProfScope prof(B200R_K_VOXEL_SURFACE, st);
-        k_voxelize_surface<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(faces, voxels, batch_size, num_faces, voxel_size);
-    }
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_voxelize_surface");
-    return 0;
+    return b200r_launch("k_voxelize_surface", B200R_K_VOXEL_SURFACE, k_voxelize_surface, (unsigned)((total + 255) / 256), 256, 0, st,
+                        faces, voxels, batch_size, num_faces, voxel_size);
 }
 
 extern "C" int b200r_voxelize_fill(int32_t* voxels, void* workspace, size_t workspace_bytes, int batch_size, int voxel_size,
@@ -299,19 +293,9 @@ extern "C" int b200r_voxelize_fill(int32_t* voxels, void* workspace, size_t work
     uint32_t* E = (uint32_t*)workspace;
     uint32_t* V = E + (size_t)rows * W;
     const unsigned row_blocks = (unsigned)((rows + 7) / 8);   // 8 warps of 256 threads, one row each
-    {
-        B200rProfScope prof(B200R_K_VOXEL_FILL, st);
-        k_voxel_pack<<<row_blocks, 256, 0, st>>>(voxels, E, V, rows, vs, W);
-    }
-    {
-        B200rProfScope prof(B200R_K_VOXEL_FILL, st);
-        k_voxel_propagate<<<batch_size, 1024, 0, st>>>(E, V, vs, W);
-    }
-    {
-        B200rProfScope prof(B200R_K_VOXEL_FILL, st);
-        k_voxel_unpack<<<row_blocks, 256, 0, st>>>(V, voxels, rows, vs, W);
-    }
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return b200r_cuda_fail(e, "k_voxel_fill");
-    return 0;
+    if (int rc = b200r_launch("k_voxel_pack", B200R_K_VOXEL_FILL, k_voxel_pack, row_blocks, 256, 0, st, voxels, E, V, rows, vs, W))
+        return rc;
+    if (int rc = b200r_launch("k_voxel_propagate", B200R_K_VOXEL_FILL, k_voxel_propagate, batch_size, 1024, 0, st, E, V, vs, W))
+        return rc;
+    return b200r_launch("k_voxel_unpack", B200R_K_VOXEL_FILL, k_voxel_unpack, row_blocks, 256, 0, st, V, voxels, rows, vs, W);
 }

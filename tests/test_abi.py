@@ -66,6 +66,24 @@ def test_bindings_match_the_c_types(lib):
         assert (fn.restype, fn.argtypes) == (restype, argtypes), name
 
 
+def test_every_kernel_launch_goes_through_the_launcher():
+    """b200r_launch (csrc/api_util.cuh) is the only place that launches a kernel, times it, counts it and checks the
+    launch; a translation unit that launched on its own would drift from b200r_launch_count and the profiler."""
+    csrc = os.path.join(ROOT, "jrender_b200", "csrc")
+    sources = [f for f in sorted(os.listdir(csrc)) if f.endswith((".cu", ".cuh")) and not f.startswith("api_util.")]
+    assert "softras_api.cu" in sources and "nmr_kernels.cuh" in sources
+    for f in sources:
+        src = open(os.path.join(csrc, f)).read()
+        for token in ("<<<", "cudaGetLastError", "B200rProfScope", "b200r_count_launch", "b200r_prof_begin", "b200r_prof_end"):
+            assert token not in src, "%s: %s" % (f, token)
+
+
+def test_retired_scheduling_option_is_unknown(lib):
+    """The forward always runs the persistent grid over the cost-ordered block queue; there is no option to turn it off."""
+    assert lib.b200r_set_option(b"softras_fwd_persistent", 0) == -1
+    assert b"unknown option" in lib.b200r_last_error()
+
+
 def test_header_parser_rejects_what_it_cannot_bind():
     from jrender_b200 import _lib
     sigs = _lib.parse_header("/* B200R_API int b200r_commented(double x); */\n#define B200R_API\n"

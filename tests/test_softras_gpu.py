@@ -273,26 +273,19 @@ def test_against_reference_kernels_on_gpu(cuda_device, nfaces, H, min_same, grad
         assert np.abs(a[m] - b[m]).sum() / np.abs(a[m]).sum() <= grad_l1, k
 
 
-def test_scheduling_choice_gives_identical_results(cuda_device):
-    """The persistent cost-ordered block queue is a pure scheduling choice: one CTA per block (queue off) must give
-    bit-identical outputs, also with T > 1 textures and a sigma large enough that every face covers every block."""
-    from jrender_b200 import _lib
+def test_cost_ordered_block_queue_matches_oracle(cuda_device):
+    """The forward's persistent grid takes its blocks from the cost-ordered queue in whatever order the warps reach it;
+    ids and colours must match the oracle, also with T > 1 textures and a sigma large enough that every face covers
+    every block."""
     fv, tex = wl.make_scene(3280, batch=2)
     P = osr.Params(image_size=200, sigma_val=3e-5)
     fv5, tex5 = wl.make_scene(280, batch=1, texture_res=3)
     P5 = osr.Params(image_size=96, sigma_val=1e-3, gamma_val=1e-3)
-    base = run_cuda(fv, tex, P, want_faces_info=False)
-    base5 = run_cuda(fv5, tex5, P5, want_faces_info=False)
-    try:
-        _lib.set_option("softras_fwd_persistent", 0)
-        got = run_cuda(fv, tex, P, want_faces_info=False)
-        got5 = run_cuda(fv5, tex5, P5, want_faces_info=False)
-    finally:
-        _lib.set_option("softras_fwd_persistent", 1)
-    for k in ("soft_colors", "aggrs_info", "faces_id_buffer"):
-        assert np.array_equal(base[k], got[k]) and np.array_equal(base5[k], got5[k]), k
+    got = run_cuda(fv, tex, P, want_faces_info=False)
+    got5 = run_cuda(fv5, tex5, P5, want_faces_info=False)
     ref = run_oracle(fv, tex, P)
     assert np.array_equal(ref["faces_id_buffer"], got["faces_id_buffer"])
+    assert np.abs(ref["soft_colors"] - got["soft_colors"]).max() <= COLOR_ATOL
     ref5 = run_oracle(fv5, tex5, P5)
     assert np.array_equal(ref5["faces_id_buffer"], got5["faces_id_buffer"])
     assert np.abs(ref5["soft_colors"] - got5["soft_colors"]).max() <= COLOR_ATOL
