@@ -38,20 +38,13 @@ struct BwdPixel {
 // Gradient contribution of one (pixel, face) pair: gv[k*3+l] = d/d vertex k coord l; gt = texture
 // gradient (T == 1 surface: gt[0..2]; vertex: gt[j*3+k]).  For surface textures with T > 1 the hit
 // texel index is returned in texel_out and gt[0..2] holds its gradient.  (:1240-1358)
-// OPT (only with !EXACT): every division is the branch-free optimistic flavour (exact_math.cuh, DivGuard) and
-// `guard.ok` says whether all of them were in range; the caller re-runs the pair with OPT = false otherwise.
-template <int DIST, int RGB, bool EXACT, bool OPT = false>
+// The DivPolicy dp gives every division its flavour; every quotient here is relaxed.  Under an optimistic policy
+// dp.ok() says afterwards whether all of them were in range; the caller re-runs the pair with a guarded one otherwise.
+template <int DIST, int RGB, class Div>
 __device__ __forceinline__ void pair_gradient(const FaceRec* rec, int fn, const BwdPixel& px, const SoftRasParams& P,
-                                              const DivConst& dc, float nmf, float r_nmf, bool s_nmf,
-                                              const float* __restrict__ tex, float gv[9], float gt[9], int& texel_out,
-                                              DivGuard& guard) {
-    static_assert(!(OPT && EXACT), "the optimistic divisions replace the relaxed ones only");
-    auto by_sigma = [&](float a) -> float { if constexpr (OPT) return dc.by_sigma_o(a, guard); else return dc.template by_sigma_t<EXACT>(a); };
-    auto by_gamma = [&](float a) -> float { if constexpr (OPT) return dc.by_gamma_o(a, guard); else return dc.template by_gamma_t<EXACT>(a); };
-    auto by_span = [&](float a) -> float { if constexpr (OPT) return dc.by_span_o(a, guard); else return dc.template by_span_t<EXACT>(a); };
-    auto dv = [&](float a, float b, float r, bool safe) -> float { if constexpr (OPT) return optimistic_div(a, b, r, safe, guard); else return div_t<EXACT>(a, b, r, safe); };
-    auto dvar = [&](float a, float b) -> float { if constexpr (OPT) return optimistic_div_var(a, b, guard); else return div_var_t<EXACT>(a, b); };
-    auto sigmoid = [&](float x) -> float { if constexpr (OPT) return sigmoid_from_negarg_opt(x, guard); else return sigmoid_from_negarg<EXACT>(x); };
+                                              Div& dp, float nmf, float r_nmf, bool s_nmf,
+                                              const float* __restrict__ tex, float gv[9], float gt[9], int& texel_out) {
+    constexpr bool EXACT = Div::kExact;
     const float* f = rec->v;
     const float xp = px.xp, yp = px.yp;
     const int T = P.T;
@@ -64,11 +57,11 @@ __device__ __forceinline__ void pair_gradient(const FaceRec* rec, int fn, const 
     } else if (DIST == 1) {
         dis = barycentric_p2f_distance(w);
         t[0] = w[0]; t[1] = w[1]; t[2] = w[2];
-        soft_fragment = sigmoid(by_sigma(-dis));
+        soft_fragment = dp.sigmoid(dp.by_sigma(-dis));
     } else {
-        sign = euclidean_p2f_distance<EXACT>(dis_x, dis_y, t, w, rec, xp, yp, OPT ? &guard : nullptr);
+        sign = euclidean_p2f_distance<false>(dis_x, dis_y, t, w, rec, xp, yp, dp);
         dis = dis_x * dis_x + dis_y * dis_y;
-        soft_fragment = sigmoid(by_sigma(-sign * dis));
+        soft_fragment = dp.sigmoid(dp.by_sigma(-sign * dis));
     }
 
     float C_grad_xy = 0.f;
@@ -83,15 +76,13 @@ __device__ __forceinline__ void pair_gradient(const FaceRec* rec, int fn, const 
             const double prod = px.d_galpha * (px.d_one_minus_alpha / den);
             C_grad_xy_alpha = d_midrange(prod) ? d2f_mid(prod) : (float)prod;
         } else {
-            C_grad_xy_alpha = C_grad_xy_alpha * dvar(1.f - px.oc[3], fmaxf(omd, 1e-6f));
+            C_grad_xy_alpha = C_grad_xy_alpha * dp.var(1.f - px.oc[3], fmaxf(omd, 1e-6f));
         }
     }
     C_grad_xy += C_grad_xy_alpha;
 
     const float w0[3] = {w[0], w[1], w[2]};
-    float zp;
-    if constexpr (OPT) zp = clip_and_z_opt(w, rec, guard);
-    else zp = clip_and_z<EXACT>(w, rec);
+    const float zp = clip_and_z<false>(w, rec, dp);
 
     if (RGB == 0) {
         if ((float)fn == px.softmax_max) {  // :1300 (int vs float compare, Q10)
@@ -107,8 +98,8 @@ __device__ __forceinline__ void pair_gradient(const FaceRec* rec, int fn, const 
         }
     } else if (RGB == 1) {
         float C_grad_xyz_rgb = 0.f;
-        const float zp_norm = by_span(P.far_ - zp);
-        const float zp_softmax = dv(soft_fragment * expf(by_gamma(zp_norm - px.softmax_max)), px.softmax_sum, px.r_ssum, px.s_ssum);
+        const float zp_norm = dp.by_span(P.far_ - zp);
+        const float zp_softmax = dp.relaxed(soft_fragment * expf(dp.by_gamma(zp_norm - px.softmax_max)), px.softmax_sum, px.r_ssum, px.s_ssum);
         float col[3];
         if (P.tex_type == 0) {
             const int j = surface_texel(w, P.R);
@@ -132,19 +123,19 @@ __device__ __forceinline__ void pair_gradient(const FaceRec* rec, int fn, const 
 #pragma unroll
         for (int k = 0; k < 3; k++) C_grad_xyz_rgb += px.g[k] * (col[k] - px.oc[k]);
         C_grad_xyz_rgb *= zp_softmax;
-        C_grad_xy += dvar(C_grad_xyz_rgb, soft_fragment);
+        C_grad_xy += dp.var(C_grad_xyz_rgb, soft_fragment);
 
-        const float C_grad_z_rgb = dv(by_gamma(C_grad_xyz_rgb), nmf, r_nmf, s_nmf) * zp * zp;
+        const float C_grad_z_rgb = dp.relaxed(dp.by_gamma(C_grad_xyz_rgb), nmf, r_nmf, s_nmf) * zp * zp;
         const uint32_t fl = rec->flags;
 #pragma unroll
         for (int k = 0; k < 3; k++) {
             const bool sz = (fl & (16u << k)) != 0;
             const float z = f[3 * k + 2], rz = rec->rz[k];
-            gv[k * 3 + 2] = dv(dv(C_grad_z_rgb * w[k], z, rz, sz), z, rz, sz);
+            gv[k * 3 + 2] = dp.relaxed(dp.relaxed(C_grad_z_rgb * w[k], z, rz, sz), z, rz, sz);
         }
     }
 
-    C_grad_xy *= by_sigma(soft_fragment * (1.f - soft_fragment));  // :1336
+    C_grad_xy *= dp.by_sigma(soft_fragment * (1.f - soft_fragment));  // :1336
     if (DIST == 1) {  // backward_barycentric_p2f_distance (:1118-1132), w := t (unclipped)
         const int pm = t[0] > t[1] ? (t[1] > t[2] ? 2 : 1) : (t[0] > t[2] ? 2 : 0);
         const float* inv = rec->inv;
@@ -279,20 +270,17 @@ k_softras_backward_lane(const SoftRasParams P, const FaceRec* __restrict__ recs,
         float gv[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         float gt[9] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
         int texel;
-        DivGuard guard;
-        guard.ok = consts_ok;   // launch-constant denominators (sigma, gamma, far - near) validated once per thread
+        DivPolicy<EXACT, !EXACT> dp(dc, consts_ok);   // !EXACT: every division branch-free, one range flag for the pair
         if (fn < 0) {
             texel = 0;   // idle lane: contributes nothing, only takes part in the shuffles below
-        } else if constexpr (!EXACT) {
-            // all divisions branch-free; one range flag for the whole pair, one (cold) re-run if it dropped
-            pair_gradient<DIST, RGB, false, true>(rec, fn, px, P, dc, nmf, r_nmf, s_nmf, btex + (size_t)fn * T * 3, gv, gt, texel, guard);
-            if (!guard.ok) {
+        } else {
+            pair_gradient<DIST, RGB>(rec, fn, px, P, dp, nmf, r_nmf, s_nmf, btex + (size_t)fn * T * 3, gv, gt, texel);
+            if (!dp.ok()) {   // cold: one re-run with the guarded divisions
 #pragma unroll
                 for (int c = 0; c < 9; c++) { gv[c] = 0.f; gt[c] = 0.f; }
-                pair_gradient<DIST, RGB, false, false>(rec, fn, px, P, dc, nmf, r_nmf, s_nmf, btex + (size_t)fn * T * 3, gv, gt, texel, guard);
+                DivPolicy<false, false> guarded(dc, consts_ok);
+                pair_gradient<DIST, RGB>(rec, fn, px, P, guarded, nmf, r_nmf, s_nmf, btex + (size_t)fn * T * 3, gv, gt, texel);
             }
-        } else {
-            pair_gradient<DIST, RGB, EXACT, false>(rec, fn, px, P, dc, nmf, r_nmf, s_nmf, btex + (size_t)fn * T * 3, gv, gt, texel, guard);
         }
         int key = fn;
         if (merge_ok) {

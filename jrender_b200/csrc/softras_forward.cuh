@@ -127,87 +127,30 @@ __device__ __forceinline__ void topk_insert(PixState& st, float zp, int fn, int 
     }
 }
 
-// The reference's per-face loop body (:318-420) for one (pixel, face) pair whose pixel is
-// inside the face's check_border rectangle.
-template <int DIST, int RGB, bool EXACT>
-__device__ __forceinline__ void shade_face(const FaceRec* rec, PixState& st, const SoftRasParams& P, const DivConst& dc,
-                                           float xp, float yp, float threshold, float* s_qz, int* s_qid, int tid,
-                                           const float* __restrict__ btex) {
-    float w[3];
-    barycentric_coordinate(w, xp, yp, rec->inv);
-
-    float soft_fragment;
-    if (DIST == 0) {
-        if (!check_pixel_inside(w)) return;  // :332-333
-        soft_fragment = 1.f;
-    } else if (DIST == 1) {
-        const float dis = barycentric_p2f_distance(w);
-        if (-dis >= threshold) return;  // :337
-        soft_fragment = sigmoid_from_negarg<EXACT>(dc.template by_sigma_t<EXACT>(-dis));
-    } else {
-        float dis_x, dis_y, t[3];
-        const float sign = euclidean_p2f_distance(dis_x, dis_y, t, w, rec, xp, yp);
-        const float dis = dis_x * dis_x + dis_y * dis_y;
-        if (sign < 0.f && dis >= threshold) return;  // :343
-        soft_fragment = sigmoid_from_negarg<EXACT>(dc.template by_sigma_t<EXACT>(-sign * dis));
-    }
-
-    // alpha aggregation, before any z test (:349-358, Q2)
-    if (P.alpha_func == 0) {
+// alpha aggregation, before any z test (:349-358, Q2)
+template <class Div>
+__device__ __forceinline__ void aggregate_alpha(PixState& st, int alpha_func, float soft_fragment, Div& dp) {
+    if (alpha_func == 0) {
         if (soft_fragment > 0.5f) st.alpha = 1.f;
-    } else if (P.alpha_func == 1) {
+    } else if (alpha_func == 1) {
         st.alpha += soft_fragment;
     } else {
-        st.alpha = alpha_prod_t<EXACT>(st.alpha, soft_fragment);
-    }
-
-    float wc[3] = {w[0], w[1], w[2]};
-    const float zp = clip_and_z(wc, rec);          // barycentric_clip :363 + zp :364
-    if (zp < P.near_ || zp > P.far_) return;       // :365
-
-    const int fn = (int)rec->face_id;
-    topk_insert(st, zp, fn, P.K, s_qz, s_qid, tid);   // s_qz = this pixel's depth list
-
-    const bool front = (rec->flags & 8u) != 0;
-    if (RGB == 0) {  // :390-397
-        if (zp < st.depth_min && check_pixel_inside(w) && (P.double_side || front)) {
-            st.depth_min = zp;
-            st.face_index_min = fn;
-            float col[3];
-            sample_texture_fwd(col, btex, fn, P.T, wc, P.R, P.tex_type, rec, zp);
-            st.sc0 = col[0]; st.sc1 = col[1]; st.sc2 = col[2];
-        }
-    } else if (RGB == 1) {  // :399-419
-        if (front || P.double_side) {
-            const float zp_norm = dc.template by_span_t<EXACT>(P.far_ - zp);
-            float exp_delta_zp = 1.f;
-            if (zp_norm > st.softmax_max) {
-                exp_delta_zp = expf(dc.template by_gamma_t<EXACT>(st.softmax_max - zp_norm));
-                st.softmax_max = zp_norm;
-            }
-            const float exp_z = expf(dc.template by_gamma_t<EXACT>(zp_norm - st.softmax_max));
-            st.softmax_sum = exp_delta_zp * st.softmax_sum + exp_z * soft_fragment;
-            float col[3];
-            sample_texture_fwd(col, btex, fn, P.T, wc, P.R, P.tex_type, rec, zp);
-            st.sc0 = exp_delta_zp * st.sc0 + exp_z * soft_fragment * col[0];
-            st.sc1 = exp_delta_zp * st.sc1 + exp_z * soft_fragment * col[1];
-            st.sc2 = exp_delta_zp * st.sc2 + exp_z * soft_fragment * col[2];
-        }
+        st.alpha = dp.alpha_prod(st.alpha, soft_fragment);
     }
 }
 
-// shade_face with every division in its branch-free optimistic form (exact_math.cuh, DivGuard): the pair's
-// arithmetic up to the first state update runs without a single range branch, the range conditions are AND-ed
-// into one flag, and a pair whose flag dropped (practically never) is handed to shade_face above before anything
-// was committed.  With the flag up every intermediate equals shade_face<.., EXACT = false>'s bit for bit:
-// same Markstein sequences, and the two exp() of the online softmax collapse into one because
-// exp((max - z)/gamma) and exp((z - max)/gamma) are never both different from 1.
-template <int DIST, int RGB>
-__device__ __forceinline__ void shade_face_opt(const FaceRec* rec, PixState& st, const SoftRasParams& P, const DivConst& dc,
-                                               float xp, float yp, float threshold, float* s_qz, int* s_qid, int tid,
-                                               const float* __restrict__ btex, bool consts_ok) {
-    DivGuard g;
-    g.ok = consts_ok;   // dc.consts_ok(), evaluated once per thread by the kernel
+// The reference's per-face loop body (:318-420) for one (pixel, face) pair whose pixel is
+// inside the face's check_border rectangle; DivPolicy<EXACT, OPT> gives every division its flavour.
+// OPT: the pair's arithmetic up to the first state update runs without a single range branch, and a
+// pair whose guard dropped (practically never) is re-run through <DIST, RGB, false, false> before
+// anything was committed.  The OPT body also collapses the two exp() of the online softmax into one:
+// exp((max - z)/gamma) and exp((z - max)/gamma) are never both different from 1 for a finite zp_norm.
+// The guarded body keeps both, as it is the one that sees a non-finite zp_norm.
+template <int DIST, int RGB, bool EXACT, bool OPT>
+__device__ __forceinline__ void shade_face(const FaceRec* rec, PixState& st, const SoftRasParams& P, const DivConst& dc,
+                                           float xp, float yp, float threshold, float* s_qz, int* s_qid, int tid,
+                                           const float* __restrict__ btex, bool consts_ok) {
+    DivPolicy<EXACT, OPT> dp(dc, consts_ok);   // consts_ok = dc.consts_ok(), evaluated once per thread by the kernel
     float w[3];
     barycentric_coordinate(w, xp, yp, rec->inv);
 
@@ -217,35 +160,31 @@ __device__ __forceinline__ void shade_face_opt(const FaceRec* rec, PixState& st,
     } else if (DIST == 1) {
         const float dis = barycentric_p2f_distance(w);
         if (-dis >= threshold) return;  // :337
-        soft_fragment = sigmoid_from_negarg_opt(dc.by_sigma_o(-dis, g), g);
+        soft_fragment = dp.sigmoid(dp.by_sigma(-dis));
     } else {
         float dis_x, dis_y, t[3];
-        const float sign = euclidean_p2f_distance<true>(dis_x, dis_y, t, w, rec, xp, yp, &g);
+        const float sign = euclidean_p2f_distance<true>(dis_x, dis_y, t, w, rec, xp, yp, dp);
         const float dis = dis_x * dis_x + dis_y * dis_y;
-        if (sign < 0.f && dis >= threshold && g.ok) return;  // :343 (an out-of-range pair falls through to the re-run)
-        soft_fragment = sigmoid_from_negarg_opt(dc.by_sigma_o(-sign * dis, g), g);
+        if (sign < 0.f && dis >= threshold && dp.ok()) return;  // :343 (OPT: an out-of-range pair falls through to the re-run)
+        soft_fragment = dp.sigmoid(dp.by_sigma(-sign * dis));
     }
+
+    if constexpr (!OPT) aggregate_alpha(st, P.alpha_func, soft_fragment, dp);
 
     float wc[3] = {w[0], w[1], w[2]};
-    const float zp = clip_and_z_opt<true>(wc, rec, g);  // barycentric_clip :363 + zp :364
+    const float zp = clip_and_z<true>(wc, rec, dp);  // barycentric_clip :363 + zp :364
     float zp_norm = 0.f, dz = 0.f, ex = 1.f;
-    if (RGB == 1) {
-        zp_norm = dc.by_span_o(P.far_ - zp, g);
-        dz = zp_norm - st.softmax_max;
-        ex = expf(dc.by_gamma_o(-fabsf(dz), g));   // = exp_delta_zp when dz > 0, exp_z otherwise (:402-407)
-    }
-    if (!g.ok) {  // cold: nothing has been committed yet
-        shade_face<DIST, RGB, false>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, tid, btex);
-        return;
-    }
-
-    // alpha aggregation, before any z test (:349-358, Q2); the default ('prod') is tested first
-    if (P.alpha_func == 2) {
-        st.alpha = st.alpha * (1.f - soft_fragment);
-    } else if (P.alpha_func == 1) {
-        st.alpha += soft_fragment;
-    } else {
-        if (soft_fragment > 0.5f) st.alpha = 1.f;
+    if constexpr (OPT) {
+        if (RGB == 1) {
+            zp_norm = dp.by_span(P.far_ - zp);
+            dz = zp_norm - st.softmax_max;
+            ex = expf(dp.by_gamma(-fabsf(dz)));   // = exp_delta_zp when dz > 0, exp_z otherwise (:402-407)
+        }
+        if (!dp.ok()) {  // cold: nothing has been committed yet
+            shade_face<DIST, RGB, false, false>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, tid, btex, consts_ok);
+            return;
+        }
+        aggregate_alpha(st, P.alpha_func, soft_fragment, dp);
     }
     if (zp < P.near_ || zp > P.far_) return;       // :365
 
@@ -263,10 +202,20 @@ __device__ __forceinline__ void shade_face_opt(const FaceRec* rec, PixState& st,
         }
     } else if (RGB == 1) {  // :399-419
         if (front || P.double_side) {
-            const bool up = dz > 0.f;            // zp_norm > softmax_max
-            const float exp_delta_zp = up ? ex : 1.f;
-            const float exp_z = up ? 1.f : ex;   // exp(0 / gamma) == 1 exactly
-            if (up) st.softmax_max = zp_norm;
+            float exp_delta_zp = 1.f, exp_z;
+            if constexpr (OPT) {
+                const bool up = dz > 0.f;        // zp_norm > softmax_max
+                exp_delta_zp = up ? ex : 1.f;
+                exp_z = up ? 1.f : ex;           // exp(0 / gamma) == 1 exactly
+                if (up) st.softmax_max = zp_norm;
+            } else {
+                zp_norm = dp.by_span(P.far_ - zp);
+                if (zp_norm > st.softmax_max) {
+                    exp_delta_zp = expf(dp.by_gamma(st.softmax_max - zp_norm));
+                    st.softmax_max = zp_norm;
+                }
+                exp_z = expf(dp.by_gamma(zp_norm - st.softmax_max));
+            }
             st.softmax_sum = exp_delta_zp * st.softmax_sum + exp_z * soft_fragment;
             float col[3];
             sample_texture_fwd(col, btex, fn, P.T, wc, P.R, P.tex_type, rec, zp);
@@ -275,15 +224,6 @@ __device__ __forceinline__ void shade_face_opt(const FaceRec* rec, PixState& st,
             st.sc2 = exp_delta_zp * st.sc2 + exp_z * soft_fragment * col[2];
         }
     }
-}
-
-// EXACT (softras_exact_tail = 1) keeps the reference's double-precision tails and the strictly guarded divisions.
-template <int DIST, int RGB, bool EXACT>
-__device__ __forceinline__ void shade_pair(const FaceRec* rec, PixState& st, const SoftRasParams& P, const DivConst& dc,
-                                           float xp, float yp, float threshold, float* s_qz, int* s_qid, int tid,
-                                           const float* __restrict__ btex, bool consts_ok) {
-    if constexpr (!EXACT) shade_face_opt<DIST, RGB>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, tid, btex, consts_ok);
-    else shade_face<DIST, RGB, EXACT>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, tid, btex);
 }
 
 // Anti-aliasing epilogue (SoftRasterizer.execute renders at 2x and mean-pools 2x2, rasterizer.py:45,54-55): the 2x2 means
@@ -502,7 +442,8 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
                     if (mask != 0u) {
                         const FaceRec* rec = &S.rec[__ffs(mask) - 1].r;
                         mask &= mask - 1u;
-                        shade_pair<DIST, RGB, EXACT>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, lane, btex, consts_ok);
+                        // EXACT (softras_exact_tail = 1): the reference's double-precision tails, guarded divisions
+                        shade_face<DIST, RGB, EXACT, !EXACT>(rec, st, P, dc, xp, yp, threshold, s_qz, s_qid, lane, btex, consts_ok);
                     }
                 }
                 head += m;
