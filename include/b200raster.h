@@ -20,6 +20,11 @@
  *   b200r_nmr_backward      <- jrender/renderer/dr/n3mr/cuda/rasterize.py:342-648, :650-727,
  *                              :729-822 (backward_pixel_map, backward_textures,
  *                              backward_depth_map), called from n3mr.py:29-67.
+ *   b200r_vol_composite_forward / _backward  <- jrender_vol/integrator/integrator.py:18-39 (about 15 elementwise ops and
+ *                              their autograd)
+ *   b200r_vol_resample      <- jrender_vol/integrator/sample.py:28-57 and jrender_vol/rayMarching/rayMarching.py:65-71
+ *                              (mids, sample_pdf, argsort of the concat)
+ *   (the other entry points name their reference code in their own comments below)
  *
  * Conventions
  *   - All tensor pointers are DEVICE pointers owned by the caller (contiguous, fp32 /
@@ -285,6 +290,40 @@ B200R_API int b200r_surface_lighting_backward(const float* vertices, const int32
                                               float ambient_intensity, const float* ambient_color, float directional_intensity,
                                               const float* directional_color, const float* direction, int with_specular, void* stream);
 
+/* ---- NeRF volume rendering (jrender_vol) -------------------------------------------------------------------------
+ * One warp per ray; no atomics, no host synchronisation, no workspace.  Every ray holds at most B200R_VOL_MAX_SAMPLES
+ * samples (S for compositing, S + Ni for resampling); beyond that the calls return B200R_EUNSUPPORTED.  num_rays 0 is a
+ * no-op.  Device pointers, float32, contiguous.
+ *
+ * b200r_vol_composite_forward replaces integrator() (jrender_vol/integrator/integrator.py:5-39):
+ *   raw [N, S, C] (C >= 4; channels 0-2 colour logits, 3 density, the rest ignored), z_vals [N, S], rays_d [N, 3],
+ *   noise [N, S] already scaled by raw_noise_std, or NULL -> rgb_map [N, 3], disp_map [N], acc_map [N], weights [N, S],
+ *   depth_map [N].  The reference's float32 expressions unfused: last interval 1e10 * |d|, alpha = 1 - exp(-relu(sigma +
+ *   noise) dist), exclusive product of (1 - alpha) + 1e-10.  disp = 1 / max(1e-10, depth / acc) with jt.maximum read as
+ *   std::max(1e-10, q), which does not propagate NaN: a ray with acc == 0 gets disp = 1e10, not NaN.
+ * b200r_vol_composite_backward: the gradient of those five outputs (each upstream gradient may be NULL = zero) with
+ *   respect to raw, written to grad_raw [N, S, C] (channels >= 4 zero).  acc_map / depth_map are the forward's (needed
+ *   with grad_disp_map).  Nothing flows to z_vals, rays_d or noise; disp passes gradient only where 1e-10 < depth / acc.
+ * b200r_vol_resample replaces sample_pdf() (jrender_vol/integrator/sample.py:28-57) and the fine stage of render_rays
+ *   (jrender_vol/rayMarching/rayMarching.py:65-71): weights + 1e-5, cdf, searchsorted(right=True), denom < 1e-5 -> 1.
+ *   u [N, Ni] uniform draws, or NULL for det (u = linspace(0, 1, Ni)).  Two shapes of call:
+ *     fine stage:  z_vals [N, S] (num_bins = S >= 2), weights [N, S] the coarse weights; bins are the mids of z_vals and
+ *                  the pdf uses weights[:, 1:S-1].  Writes z_samples [N, Ni] and z_vals_fine [N, S + Ni], the ascending
+ *                  sort of the concatenation (NaN last).  bins must be NULL.
+ *     sample_pdf:  bins [N, num_bins] (>= 1), weights [N, num_bins - 1]; z_vals and z_vals_fine NULL; writes z_samples. */
+#define B200R_VOL_MAX_SAMPLES 1024
+B200R_API int b200r_vol_composite_forward(const float* raw, const float* z_vals, const float* rays_d, const float* noise,
+                                          float* rgb_map, float* disp_map, float* acc_map, float* weights, float* depth_map,
+                                          int num_rays, int num_samples, int raw_channels, int white_bkgd, void* stream);
+B200R_API int b200r_vol_composite_backward(const float* raw, const float* z_vals, const float* rays_d, const float* noise,
+                                           const float* acc_map, const float* depth_map, const float* grad_rgb_map,
+                                           const float* grad_disp_map, const float* grad_acc_map, const float* grad_weights,
+                                           const float* grad_depth_map, float* grad_raw, int num_rays, int num_samples,
+                                           int raw_channels, int white_bkgd, void* stream);
+B200R_API int b200r_vol_resample(const float* z_vals, const float* bins, const float* weights, const float* u,
+                                 float* z_samples, float* z_vals_fine, int num_rays, int num_bins, int num_importance,
+                                 void* stream);
+
 /* Launch counter: number of kernels this library has launched in this process
  * (bench.py reports the delta over the timed region as "gpu_launches"). */
 B200R_API unsigned long long b200r_launch_count(void);
@@ -307,7 +346,8 @@ enum { B200R_K_FACE_SETUP = 0, B200R_K_COARSE_BIN = 1, B200R_K_SOFTRAS_FWD = 2, 
        B200R_K_NMR_BWD_MAPS = 8, B200R_K_SOFTRAS_BWD_FINALIZE = 9, B200R_K_NMR_PACK = 10,
        B200R_K_PROJECT_FWD = 11, B200R_K_PROJECT_BWD = 12, B200R_K_FLATTEN_LOSS = 13, B200R_K_LAPLACIAN_LOSS = 14,
        B200R_K_LIGHTING = 15, B200R_K_BAKE = 16, B200R_K_ATLAS = 17, B200R_K_VOXEL_SURFACE = 18,
-       B200R_K_VOXEL_FILL = 19, B200R_K_CHUNK_RECTS = 20, B200R_K_DEBUG = 21, B200R_K_COUNT };
+       B200R_K_VOXEL_FILL = 19, B200R_K_CHUNK_RECTS = 20, B200R_K_DEBUG = 21, B200R_K_VOL_COMPOSITE_FWD = 22,
+       B200R_K_VOL_COMPOSITE_BWD = 23, B200R_K_VOL_RESAMPLE = 24, B200R_K_COUNT };
 B200R_API void b200r_profile_enable(int on);
 B200R_API void b200r_profile_reset(void);
 B200R_API int b200r_profile_read(int kernel, double* total_ms, long long* launches);
