@@ -30,7 +30,7 @@ struct __align__(16) FaceRec {
     uint32_t rect_x;   // x0 | x1 << 16 : pixel columns passing check_border (inclusive)
     uint32_t rect_r;   // r0 | r1 << 16 : output rows passing check_border (inclusive, row 0 = top)
     uint32_t flags;    // bit k (k<3): face_obt[k]; bit 3: check_face_frontside;
-                       // bit 4+k: midrange(z_k); bit 7+k: midrange(den_k)
+                       // bit 4+k: midrange(z_k) and a finite inv; bit 7+k: midrange(den_k)
     uint32_t face_id;  // index within the batch element
     float inv[9];      // face_inv  (:205-217)
     float v[9];        // x0 y0 z0 x1 y1 z1 x2 y2 z2

@@ -74,14 +74,18 @@ static __global__ void __launch_bounds__(256) k_face_setup(const float* __restri
     }
     // check_face_frontside (:37-40)
     if ((f[7] - f[1]) * (f[3] - f[0]) < (f[4] - f[1]) * (f[6] - f[0])) flags |= 8u;
-    // refined reciprocals of the per-face denominators (exact_math.cuh)
+    // refined reciprocals of the per-face denominators (exact_math.cuh).  A face whose inverse is not finite (a NaN or
+    // infinite vertex) gets no z bits, so that clip_and_z sends its pairs to the guarded body (NaN weights)
+    bool inv_finite = true;
+#pragma unroll
+    for (int k = 0; k < 9; k++) inv_finite = inv_finite && isfinite(r.inv[k]);
 #pragma unroll
     for (int k = 0; k < 3; k++) {
         const float z = f[3 * k + 2];
         const float den = r.a0[3 * k + k] - r.a0[3 * k + (k + 1) % 3];
         r.rz[k] = rcp_refined(z);
         r.rden[k] = rcp_refined(den);
-        if (midrange(z)) flags |= 16u << k;
+        if (midrange(z) && inv_finite) flags |= 16u << k;
         if (midrange(den)) flags |= 128u << k;
     }
     r.flags = flags;
