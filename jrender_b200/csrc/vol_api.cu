@@ -235,7 +235,7 @@ k_vol_resample(const float* __restrict__ z_vals, const float* __restrict__ bins_
     if (z_vals) {
         const float* zr = z_vals + ray * S;
         for (int k = lane; k < S; k += 32) buf[k] = __ldg(zr + k);
-        for (int k = S + Ni + lane; k < P; k += 32) buf[k] = INFINITY;
+        for (int k = S + Ni + lane; k < P; k += 32) buf[k] = NAN;   // sorts behind every value, NaN included
         __syncwarp();
         for (int k = lane; k < nb; k += 32) bins[k] = .5f * (buf[k + 1] + buf[k]);   // rayMarching.py:67
     } else {
@@ -271,7 +271,8 @@ k_vol_resample(const float* __restrict__ z_vals, const float* __restrict__ bins_
     }
     if (!z_vals) return;
     __syncwarp();
-    // bitonic sort of buf[0, P) ascending; NaN sorts last, as torch.sort puts it
+    // bitonic sort of buf[0, P) ascending; NaN sorts last, as torch.sort puts it.  The padding past S + Ni is NaN too, so
+    // the first S + Ni are torch.sort's: the real values in order, then as many NaNs as the merge held
     for (int size = 2; size <= P; size <<= 1) {
         for (int stride = size >> 1; stride > 0; stride >>= 1) {
             for (int i = lane; i < P / 2; i += 32) {
@@ -279,7 +280,7 @@ k_vol_resample(const float* __restrict__ z_vals, const float* __restrict__ bins_
                 const int hi = lo + stride;
                 const bool up = (lo & size) == 0;
                 const float a = buf[lo], b = buf[hi];
-                const bool gt = a > b || (isnan(a) && !isnan(b));
+                const bool gt = !(a <= b) && b == b;   // a > b, or a NaN and b not
                 if (gt == up) buf[lo] = b, buf[hi] = a;
             }
             __syncwarp();

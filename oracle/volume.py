@@ -73,9 +73,10 @@ def _exclusive_transmittance(t_tiles):
     return T
 
 
-def composite(raw, z_vals, rays_d, noise=None, white_bkgd=False):
+def composite(raw, z_vals, rays_d, noise=None, white_bkgd=False, trace=None):
     """integrator() in the kernel's order: raw [N, S, C >= 4], z_vals [N, S], rays_d [N, 3], noise [N, S] or None ->
-    dict rgb_map [N, 3], disp_map, acc_map, weights [N, S], depth_map."""
+    dict rgb_map [N, 3], disp_map, acc_map, weights [N, S], depth_map.  A dict `trace` receives the per-sample
+    intermediates [N, S]: exp_arg (what exp is taken of), alpha, t = (1 - alpha) + 1e-10 and the transmittance T."""
     raw, z, d = (np.asarray(a, F32) for a in (raw, z_vals, rays_d))
     N, S = z.shape
     norm = np.sqrt(d[:, 0] * d[:, 0] + d[:, 1] * d[:, 1] + d[:, 2] * d[:, 2])
@@ -83,10 +84,13 @@ def composite(raw, z_vals, rays_d, noise=None, white_bkgd=False):
     x = raw[..., 3]
     if noise is not None:
         x = x + np.asarray(noise, F32)
-    r = np.where(x > 0, x, F32(0))
-    alpha = F32(1) - np.exp(-r * dist)
+    r = np.where(x > 0, x, F32(0))   # relu(NaN) = 0, as the kernel's x > 0 ? x : 0
+    arg = -r * dist
+    alpha = F32(1) - np.exp(arg)
     t = (F32(1) - alpha) + F32(1e-10)
     T = _exclusive_transmittance(_tiles(t, F32(1)))
+    if trace is not None:
+        trace.update(exp_arg=arg, alpha=alpha, t=t, T=T.reshape(N, -1)[:, :S])
     w = (_tiles(alpha, F32(0)) * T)
     sig = _sigmoid(raw[..., :3])
     rgb = np.stack([_lane_sum(w * _tiles(sig[..., c], F32(0))) for c in range(3)], -1)
@@ -107,10 +111,11 @@ def linspace01(n):
     return (np.arange(n, dtype=F32) * F32(1)) / F32(n - 1) + F32(0)
 
 
-def resample(weights, n_importance, u=None, z_vals=None, bins=None):
+def resample(weights, n_importance, u=None, z_vals=None, bins=None, trace=None):
     """The resampler in the kernel's order.  Fine stage (z_vals [N, S], weights [N, S]): bins = mids, pdf of
     weights[:, 1:-1]; returns (z_samples [N, Ni], z_vals_fine [N, S + Ni]).  sample_pdf (bins [N, nb], weights
-    [N, nb - 1]): returns (z_samples, None).  u [N, Ni] or None (det)."""
+    [N, nb - 1]): returns (z_samples, None).  u [N, Ni] or None (det).  A dict `trace` receives cdf [N, nb], and per
+    sample [N, Ni] u, the searchsorted count inds and the denominator before the 1e-5 test."""
     w = np.asarray(weights, F32)
     if z_vals is not None:
         z = np.asarray(z_vals, F32)
@@ -135,6 +140,8 @@ def resample(weights, n_importance, u=None, z_vals=None, bins=None):
     g = lambda a, i: np.take_along_axis(a, i, 1)
     cdf0, cdf1, bin0, bin1 = g(cdf, below), g(cdf, above), g(bins, below), g(bins, above)
     denom = cdf1 - cdf0
+    if trace is not None:
+        trace.update(cdf=cdf, u=u, inds=inds, denom=denom)
     denom = np.where(denom < F32(1e-5), F32(1), denom)
     samples = bin0 + ((u - cdf0) / denom) * (bin1 - bin0)
     if z_vals is None:
@@ -144,14 +151,21 @@ def resample(weights, n_importance, u=None, z_vals=None, bins=None):
 
 # ---- op-by-op PyTorch mirror of the reference ---------------------------------------------------------------------
 
-def integrator_mirror(raw, z_vals, rays_d, noise=None, white_bkgd=False):
-    """integrator.py:18-39 op by op; noise is the already scaled gauss draw (or None).  Returns the five outputs."""
+def kernel_relu(x):
+    """relu as the kernels and composite() read it, x > 0 ? x : 0: NaN gives 0 (and a zero gradient), where
+    torch.relu propagates it.  Which of the two Jittor's relu is has not been confirmed (DESIGN.md section 9)."""
+    return torch.where(x > 0, x, torch.zeros_like(x))
+
+
+def integrator_mirror(raw, z_vals, rays_d, noise=None, white_bkgd=False, relu=torch.relu):
+    """integrator.py:18-39 op by op; noise is the already scaled gauss draw (or None).  Returns the five outputs.
+    relu=kernel_relu gives the kernels' reading of relu(NaN)."""
     dists = z_vals[..., 1:] - z_vals[..., :-1]
     dists = torch.cat([dists, torch.full_like(dists[..., :1], 1e10)], -1)
     dists = dists * torch.norm(rays_d.unsqueeze(-2), p=2, dim=-1)
     rgb = torch.sigmoid(raw[..., :3])
     sigma = raw[..., 3] if noise is None else raw[..., 3] + noise
-    alpha = 1. - torch.exp(-torch.relu(sigma) * dists)
+    alpha = 1. - torch.exp(-relu(sigma) * dists)
     ones = torch.ones(alpha.shape[0], 1, dtype=alpha.dtype, device=alpha.device)
     weights = alpha * torch.cumprod(torch.cat([ones, 1. - alpha + 1e-10], -1), -1)[:, :-1]
     rgb_map = torch.sum(weights.unsqueeze(-1) * rgb, -2)
