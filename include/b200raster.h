@@ -290,6 +290,37 @@ B200R_API int b200r_surface_lighting_backward(const float* vertices, const int32
                                               float ambient_intensity, const float* ambient_color, float directional_intensity,
                                               const float* directional_color, const float* direction, int with_specular, void* stream);
 
+/* ---- normal-mapped surface lighting ---------------------------------------------------------------------------------
+ * Lighting.execute's normal-map branch (jrender/renderer/lighting/lighting.py:186-204 with mesh.normal_textures, and the
+ * 4-D branch of directional_lighting.py:63-135): one normal per texel, N = normalize(n_t . TBN) (structures/mesh.py:276-284,
+ * surface_ResNormals), the face centroid as position, and per-texel metallic / roughness (not averaged).  One thread per
+ * texel forward.  Same light parameters and batch rules as b200r_surface_lighting_*; in addition
+ *   textures / out_textures [B, nf, T, 3], normal_textures [normal_batch, normal_faces, normal_texels, 3] (tangent space),
+ *   tbn [tbn_batch, tbn_faces, 3, 3] (rows T, B, N), metallic / roughness [B, nf, T] or NULL.
+ * normal_batch and tbn_batch are 1 or B; normal_faces, normal_texels and tbn_faces must equal nf and T (else B200R_EINVAL).
+ * backward overwrites each of grad_textures [B, nf, T, 3], grad_normal_textures [normal_batch, nf, T, 3] (summed over the
+ * batch when normal_batch is 1), grad_vertices [vertices_batch, nv, 3] (through the centroid only) and the per-texel
+ * grad_metallic / grad_roughness [B, nf, T] that is not NULL.  No gradient reaches the TBN.  Material gradients need
+ * metallic and roughness (else B200R_EINVAL); they are 0 where the Cook-Torrance branch is off. */
+B200R_API int b200r_normal_mapped_lighting_forward(const float* vertices, const int32_t* faces, const float* textures,
+                                                   const float* normal_textures, const float* tbn, const float* metallic,
+                                                   const float* roughness, const float* eye, float* out_textures, int B,
+                                                   int vertices_batch, int faces_batch, int eye_batch, int normal_batch,
+                                                   int normal_faces, int normal_texels, int tbn_batch, int tbn_faces, int nv, int nf,
+                                                   int T, float ambient_intensity, const float* ambient_color,
+                                                   float directional_intensity, const float* directional_color,
+                                                   const float* direction, int with_specular, void* stream);
+B200R_API int b200r_normal_mapped_lighting_backward(const float* vertices, const int32_t* faces, const float* textures,
+                                                    const float* normal_textures, const float* tbn, const float* metallic,
+                                                    const float* roughness, const float* eye, const float* grad_out,
+                                                    float* grad_textures, float* grad_normal_textures, float* grad_vertices,
+                                                    float* grad_metallic, float* grad_roughness, int B, int vertices_batch,
+                                                    int faces_batch, int eye_batch, int normal_batch, int normal_faces,
+                                                    int normal_texels, int tbn_batch, int tbn_faces, int nv, int nf, int T,
+                                                    float ambient_intensity, const float* ambient_color,
+                                                    float directional_intensity, const float* directional_color,
+                                                    const float* direction, int with_specular, void* stream);
+
 /* ---- NeRF volume rendering (jrender_vol) -------------------------------------------------------------------------
  * One warp per ray; no atomics, no host synchronisation, no workspace.  Every ray holds at most B200R_VOL_MAX_SAMPLES
  * samples (S for compositing, S + Ni for resampling); beyond that the calls return B200R_EUNSUPPORTED.  num_rays 0 is a

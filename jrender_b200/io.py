@@ -14,7 +14,9 @@ and for the export:
   jrender/io/save_obj.py:7-84                        (.obj / .mtl / .png writer; the texture atlas is painted by
                                                       b200r_texture_atlas_softras / _n3mr <- io/utils/create_texture_image.py)
 Images are read and written with OpenCV (the reference uses skimage, which is not installed here).
-Normal / bump maps and TBN (SSS, render2) are outside the hot-path scope.
+The SoftRas loader's normal-map branch (_load_obj_for_softras.py:10-15, 19-40, 120-140 and
+Scene/objects/utils/create_TBN.py) is mirrored behind load_obj(with_normal_map=True): `map_normal` images, bump maps
+converted to normal maps, the GPU bake and the per-face TBN.
 """
 import os
 
@@ -37,9 +39,11 @@ def _placed(x, dev, dtype=torch.float32):
     return t.to(device=dev, dtype=dtype).contiguous()
 
 
-def load_mtl(filename_mtl):
-    """_load_obj_for_softras.py:19-40: Kd colours and map_Kd filenames per material."""
-    texture_filenames, colors, material_name = {}, {}, ''
+def load_mtl(filename_mtl, with_normal_map=False):
+    """_load_obj_for_softras.py:19-40: Kd colours and map_Kd filenames per material.  With with_normal_map, also the
+    normal / bump map filename ('' when there is none): the third token of `map_normal <scale> <file>` (the scale is
+    ignored; the last such line wins)."""
+    texture_filenames, colors, material_name, normal_filename = {}, {}, '', ''
     with open(filename_mtl) as f:
         for line in f.readlines():
             s = line.split()
@@ -51,6 +55,12 @@ def load_mtl(filename_mtl):
                 texture_filenames[material_name] = s[1]
             if s[0] == 'Kd':
                 colors[material_name] = np.array(list(map(float, s[1:4])))
+            if s[0] == 'map_normal' and with_normal_map:
+                if len(s) < 3:
+                    raise ValueError("%s: 'map_normal <scale> <file>' expected, got %r" % (filename_mtl, line.strip()))
+                normal_filename = s[2]
+    if with_normal_map:
+        return colors, texture_filenames, normal_filename
     return colors, texture_filenames
 
 
@@ -64,6 +74,57 @@ def _imread_rgb01(path):
     else:
         img = img[:, :, :3][:, :, ::-1]   # BGR(A) -> RGB, drop alpha like the reference
     return img.astype(np.float32) / 255.
+
+
+def _imread_native01(path):
+    """A normal or bump map as the reference reads it (skimage, then / 255.): at its native bit depth, so a 16-bit image
+    reaches 65535 / 255 = 257.  Grayscale stays [H, W]; colour becomes RGB [H, W, 3] (alpha dropped)."""
+    import cv2
+    img = cv2.imread(path, cv2.IMREAD_UNCHANGED)
+    if img is None:
+        raise IOError("cannot read normal map %s" % path)
+    if img.ndim == 3:
+        img = img[:, :, :3][:, :, ::-1]   # BGR(A) -> RGB
+    return img.astype(np.float32) / 255.
+
+
+def _normalize_np(x, axis, eps):
+    """x / max(||x||_2, eps) along `axis` in float32 (jt.normalize)."""
+    x = x.astype(np.float32)
+    n = np.sqrt((x * x).sum(axis=axis, keepdims=True, dtype=np.float32)).astype(np.float32)
+    return (x / np.maximum(n, np.float32(eps))).astype(np.float32)
+
+
+def bump_to_normal_map(bump):
+    """bump_mapToNormal_map (_load_obj_for_softras.py:10-15): a grayscale height image [H, W] to a tangent-space normal
+    image [H - 2, W - 2, 3] in [0, 1]: central differences, a z component of 6, normalised with eps 1e-5, then (n + 1) / 2."""
+    b = np.asarray(bump, np.float32)
+    if b.ndim != 2 or b.shape[0] < 3 or b.shape[1] < 3:
+        raise ValueError("bump_to_normal_map: a grayscale image of at least 3 x 3 pixels expected, got %s" % (b.shape,))
+    dx = b[1:-1, :-2] - b[1:-1, 2:]
+    dy = b[:-2, 1:-1] - b[2:, 1:-1]
+    n = np.stack((-dx, -dy, np.full(dx.shape, 6, np.float32)), axis=2)
+    return ((_normalize_np(n, 2, 1e-5) + 1.) / 2.).astype(np.float32)
+
+
+def create_TBN(face_texcoords, face_wcoords):
+    """create_TBN (Scene/objects/utils/create_TBN.py): the per-face tangent frame [nf, 3, 3], rows T, B, N, from the face
+    UVs [nf, 3, 2] and world-space vertices [nf, 3, 3], in float32 in the reference's order of operations.  A face whose
+    UV triangle is degenerate divides by zero and gets a non-finite frame, as in the reference."""
+    ft, fw = np.asarray(face_texcoords, np.float32), np.asarray(face_wcoords, np.float32)
+    e1, e2 = fw[:, 0] - fw[:, 1], fw[:, 0] - fw[:, 2]
+    n = _normalize_np(np.cross(e1, e2)[:, None, :], 2, 1e-12)
+    u1, v1 = ft[:, 0, 0] - ft[:, 1, 0], ft[:, 0, 1] - ft[:, 1, 1]
+    u2, v2 = ft[:, 0, 0] - ft[:, 2, 0], ft[:, 0, 1] - ft[:, 2, 1]
+    with np.errstate(divide='ignore', invalid='ignore'):
+        denom = (1 / (u1 * v2 - u2 * v1)).astype(np.float32)[:, None, None]
+        inverse = np.stack((np.stack((v2, -v1), axis=1), np.stack((-u2, u1), axis=1)), axis=1).astype(np.float32)
+        TB = denom * np.matmul(inverse, np.stack((e1, e2), axis=1)).astype(np.float32)
+        T = TB[:, 0, :][:, None, :]
+        T = T - np.sum(T * n, axis=2)[:, None] * n
+        T = _normalize_np(T, 2, 1e-12)
+        B = _normalize_np(np.cross(n, T), 2, 1e-12)
+    return np.concatenate([T, B, n], axis=1).astype(np.float32)
 
 
 def bake_textures_for_softras(image, faces_uv, textures, is_update, device=None):
@@ -161,8 +222,29 @@ def load_textures_n3mr(filename_obj, filename_mtl, texture_res, texture_wrapping
     return textures
 
 
-def load_textures(filename_obj, filename_mtl, texture_res):
-    """_load_obj_for_softras.py:43-140 without the normal-map branch: [nf, R*R, 3] float32."""
+def load_textures(filename_obj, filename_mtl, texture_res, face_vertices=None):
+    """_load_obj_for_softras.py:43-140: [nf, R*R, 3] float32.
+
+    With face_vertices ([nf, 3, 3], the un-normalised world-space vertices of every face), also the normal-map branch:
+    returns (textures, normal_textures [nf, R*R, 3] or None, TBN [nf, 3, 3] or None, face_texcoords [nf, 3, 2]).  The
+    `map_normal` image is read at its native bit depth and divided by 255; a grayscale image is a bump map and goes
+    through bump_to_normal_map.  It is flipped, baked into every face by b200r_bake_textures_softras and mapped to unit
+    tangent-space normals by normalize(n * 2 - 1).  Unlike the reference, nothing is written next to the .obj."""
+    if face_vertices is not None:
+        textures = load_textures(filename_obj, filename_mtl, texture_res)
+        faces_uv, _ = _parse_texture_faces(filename_obj)
+        _, _, normal_filename = load_mtl(filename_mtl, with_normal_map=True)
+        if normal_filename == '':
+            return textures, None, None, faces_uv
+        image = _imread_native01(os.path.join(os.path.dirname(filename_obj), normal_filename))
+        if image.ndim == 2:
+            image = bump_to_normal_map(image)
+        TBN = create_TBN(faces_uv, face_vertices)
+        nt = bake_textures_for_softras(np.ascontiguousarray(image[::-1, :, :]), faces_uv,
+                                       np.ones((faces_uv.shape[0], texture_res ** 2, 3), np.float32),
+                                       np.ones(faces_uv.shape[0], np.int32))
+        normal_textures = _normalize_np(nt.cpu().numpy() * 2 - 1, 2, 1e-12)
+        return textures, normal_textures, TBN, faces_uv
     faces_uv, material_names = _parse_texture_faces(filename_obj)
     colors, texture_filenames = load_mtl(filename_mtl)
     textures = np.ones((faces_uv.shape[0], 3), np.float32)
@@ -179,9 +261,15 @@ def load_textures(filename_obj, filename_mtl, texture_res):
 
 
 def load_obj(filename_obj, normalization=False, load_texture=False, dr_type='softras', texture_res=4,
-             texture_type='surface', texture_wrapping='REPEAT', use_bilinear=True):
+             texture_type='surface', texture_wrapping='REPEAT', use_bilinear=True, with_normal_map=False):
     """load_obj.py:9-20 / _load_obj_for_softras.py:142-207.  Returns torch tensors:
-    (vertices [nv,3] f32, faces [nf,3] i32) or (+ textures) when load_texture."""
+    (vertices [nv,3] f32, faces [nf,3] i32) or (+ textures) when load_texture.
+
+    with_normal_map (SoftRas surface textures only): (vertices, faces, textures, normal_textures [nf, R*R, 3], TBN
+    [nf, 3, 3], face_texcoords [nf, 3, 2]), the last three None when the .mtl names no `map_normal`.  The TBN is built
+    from the vertices before normalization, as in the reference."""
+    if with_normal_map and not (load_texture and dr_type == 'softras' and texture_type == 'surface'):
+        raise ValueError("load_obj: with_normal_map needs load_texture=True, dr_type='softras', texture_type='surface'")
     assert dr_type in ['softras', 'n3mr']
     assert texture_type in ['surface', 'vertex']
     with open(filename_obj) as f:
@@ -206,9 +294,14 @@ def load_obj(filename_obj, normalization=False, load_texture=False, dr_type='sof
         if textures is None:
             raise Exception('Failed to load textures.')
     elif load_texture and texture_type == 'surface':
+        normal_map = None
         for line in lines:
             if line.startswith('mtllib'):
-                textures = load_textures(filename_obj, os.path.join(os.path.dirname(filename_obj), line.split()[1]), texture_res)
+                filename_mtl = os.path.join(os.path.dirname(filename_obj), line.split()[1])
+                if with_normal_map:
+                    textures, *normal_map = load_textures(filename_obj, filename_mtl, texture_res, face_vertices=vertices[faces])
+                else:
+                    textures = load_textures(filename_obj, filename_mtl, texture_res)
         if textures is None:
             raise Exception('Failed to load textures.')
     elif load_texture and texture_type == 'vertex':
@@ -220,6 +313,8 @@ def load_obj(filename_obj, normalization=False, load_texture=False, dr_type='sof
         vertices = vertices * 2
         vertices = vertices - vertices.max(0) / 2
     v, f = torch.from_numpy(vertices.astype(np.float32)), torch.from_numpy(faces)
+    if with_normal_map:
+        return (v, f, torch.from_numpy(textures)) + tuple(None if x is None else torch.from_numpy(x) for x in normal_map)
     if load_texture:
         return v, f, torch.from_numpy(textures)
     return v, f

@@ -2,8 +2,9 @@
 
 Holds vertices [B,nv,3], faces [B,nf,3] and textures; lazily gathers face_vertices
 [B,nf,3,3] / face_textures -- the two tensors the rasterizer consumes.  Only the attributes the
-rasterizer path (Renderer -> Lighting -> Transform -> rasterizer) reads are mirrored, plus export (save_obj) and
-voxelize; normal maps / TBN / SSS are outside the hot-path scope (SURVEY.md section 8).
+rasterizer path (Renderer -> Lighting -> Transform -> rasterizer) reads are mirrored, plus export (save_obj), voxelize
+and normal maps (normal_textures, TBN, face_texcoords, surface_ResNormals); SSS is outside the scope (SURVEY.md
+section 8).
 """
 import numpy as np
 import torch
@@ -54,11 +55,21 @@ class Mesh(object):
         self._vertex_normals_update = True
         self._with_specular = True   # mesh.py:74: lighting takes the Cook-Torrance branch by default
         self._with_SSS = with_SSS
-        self._face_texcoords = face_texcoords
         self._fill_back = False
         self.dr_type = dr_type
-        self.normal_textures = None
         dev = self._vertices.device
+        # normal map (mesh.py:77-79, 133-138): tangent-space normal textures [1, nf, T, 3] and the per-face tangent frame
+        # TBN [1, nf, 3, 3] (rows T, B, N); the face UVs [1, nf, 3, 2] ride along
+        def batched(x, dim):
+            if x is None:
+                return None
+            x = torch.from_numpy(x).float() if isinstance(x, np.ndarray) else x
+            return (x[None] if x.dim() == dim else x).to(dev)
+        if (normal_textures is None) != (TBN is None):
+            raise ValueError("Mesh: normal_textures and TBN come together")
+        self.normal_textures = batched(normal_textures, 3)
+        self.TBN = batched(TBN, 3)
+        self._face_texcoords = batched(face_texcoords, 3)
 
         if textures is None:
             if texture_type == 'surface':
@@ -168,7 +179,12 @@ class Mesh(object):
 
     @property
     def surface_normals(self):
-        """mesh.py:213-229 (float64 cross product, then normalised, back to float32)."""
+        """mesh.py:213-229 (float64 cross product, then normalised, back to float32).  With a normal map (:222-225): the
+        face's mean tangent-space normal through its TBN, normalised; recomputed on every access, so that it follows
+        normal textures being fitted."""
+        if self.normal_textures is not None:
+            mean = (torch.sum(self.normal_textures, dim=2) / self.texture_res ** 2).unsqueeze(2)
+            return F.normalize(torch.matmul(mean, self.TBN).squeeze(2), dim=2, eps=1e-12)
         if self._surface_normals_update:
             v10 = (self.face_vertices[:, :, 0] - self.face_vertices[:, :, 1]).double()
             v12 = (self.face_vertices[:, :, 2] - self.face_vertices[:, :, 1]).double()
@@ -213,6 +229,15 @@ class Mesh(object):
         self._fill_back = False
 
     @property
+    def surface_ResNormals(self):
+        """mesh.py:276-284: one world-space normal per texel [1|B, nf, T, 3], normalize(n_t . TBN) with the 1x3 by 3x3
+        matmul of the reference (the TBN broadcast over the texels rather than repeated).  None without a normal map."""
+        if self.normal_textures is None:
+            return None
+        n = torch.matmul(self.normal_textures.unsqueeze(3), self.TBN.unsqueeze(2)).squeeze(3)
+        return F.normalize(n, dim=3, eps=1e-12)
+
+    @property
     def face_texcoords(self):
         return self._face_texcoords
 
@@ -220,14 +245,20 @@ class Mesh(object):
     def from_obj(cls, filename_obj, normalization=False, load_texture=False, dr_type='softras', texture_res=1,
                  texture_type='surface', texture_wrapping='REPEAT', use_bilinear=True, with_SSS=False):
         from .io import load_obj
-        if load_texture:
+        normal_textures = TBN = face_texcoords = None
+        if load_texture and dr_type == 'softras' and texture_type == 'surface':
+            vertices, faces, textures, normal_textures, TBN, face_texcoords = load_obj(
+                filename_obj, normalization=normalization, texture_res=texture_res, load_texture=True, dr_type=dr_type,
+                texture_type=texture_type, with_normal_map=True)
+        elif load_texture:
             vertices, faces, textures = load_obj(filename_obj, normalization=normalization, texture_res=texture_res,
                                                  load_texture=True, dr_type=dr_type, texture_type=texture_type,
                                                  texture_wrapping=texture_wrapping, use_bilinear=use_bilinear)
         else:
             vertices, faces = load_obj(filename_obj, normalization=normalization, load_texture=False, dr_type=dr_type)
             textures = None
-        return cls(vertices, faces, textures, texture_res, texture_type, dr_type=dr_type, with_SSS=with_SSS)
+        return cls(vertices, faces, textures, texture_res, texture_type, dr_type=dr_type, normal_textures=normal_textures,
+                   TBN=TBN, with_SSS=with_SSS, face_texcoords=face_texcoords)
 
     def save_obj(self, filename_obj, save_texture=False, texture_res_out=16):
         """structures/mesh.py:330-338.  save_texture writes the textures too (io.save_obj): surface textures (SoftRas
@@ -258,6 +289,10 @@ class Mesh(object):
         self._textures = self._textures.to(device)
         self.metallic_textures = self.metallic_textures.to(device)
         self.roughness_textures = self.roughness_textures.to(device)
+        if self.normal_textures is not None:
+            self.normal_textures, self.TBN = self.normal_textures.to(device), self.TBN.to(device)
+        if isinstance(self._face_texcoords, torch.Tensor):
+            self._face_texcoords = self._face_texcoords.to(device)
         self._origin_vertices, self._origin_faces, self._origin_textures = self._vertices, self._faces, self._textures
         self._face_vertices_update = self._surface_normals_update = self._vertex_normals_update = True
         return self

@@ -18,6 +18,7 @@ FILES = [
     "data/obj/spot/spot_triangulated.obj", "data/obj/spot/spot_triangulated.mtl", "data/obj/spot/spot_texture.png",   # demo1-render.py:17,26
     "data/obj/sphere/sphere_1352.obj",                                                                                # demo2-deform.py:55
     "data/source.npy", "data/camera.npy",                                                                             # demo2-deform.py:50-53
+    "data/head/head.obj", "data/head/head.mtl", "data/head/lambertian.jpg", "data/head/bump.png",                      # demo1.5-SSS.py:17,23
 ]
 
 
