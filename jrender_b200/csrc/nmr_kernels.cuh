@@ -108,9 +108,10 @@ __device__ __forceinline__ bool nmr_face_pixel(const NmrFace& r, int xi, int yi,
     return zp < far_;                                                 // NaN
 }
 
-// float -> unsigned with the same order (negative depths are possible when `near` is negative)
+// float -> unsigned with the same order (negative depths are possible when `near` is negative).  -0 is mapped to +0
+// first: the oracle's `zp < depth` treats them as equal, so a tie between a -0 and a +0 face goes to the lower id.
 __device__ __forceinline__ uint32_t nmr_order_bits(float z) {
-    const uint32_t u = __float_as_uint(z);
+    const uint32_t u = __float_as_uint(z == 0.f ? 0.f : z);
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
@@ -412,8 +413,10 @@ __device__ __forceinline__ void k9_scan(const float* __restrict__ prow, const in
 //  * Every pixel of an outward scan lies strictly beyond the crossing point (d1_out = floor(d1_cross) + 1 or
 //    ceil(d1_cross) - 1, then away from it), so delta = d1 - d1_cross has ONE sign for the whole scan and the reference's
 //    per-pixel `dist = (0 < dist) ? dist + eps : dist - eps` (:510/:515) adds a per-scan constant: dist = fma(delta, k, +-eps)
-//    (|k| >= 2 / is, so delta * k never underflows; no cancellation, so |dist| >= eps and lanes past the end of the row --
-//    which evaluate a zero record -- add exactly 0).
+//    (|k| >= 2 / is, so delta * k never underflows; no cancellation, so |dist| >= eps).
+//  * Lanes past the end of the scan (only in the last trip pair) evaluate a zero record with delta replaced by `side`
+//    (d1_from - d1_cross), so their dist is nonzero and they add exactly 0.  Their own delta would not do: in a scan toward pixel 0 they sit at d1_in
+//    and beyond, across the crossing, where fma(delta, k, e) can cancel to exactly 0 -- and 0 * inf is NaN.
 //  * `diff_grad <= 0 -> continue` (:503) is max.NaN(diff, 0): a NaN still propagates like the reference's test lets it.
 //  * delta advances by 64 per trip instead of being re-formed from the pixel number (<= 1 ulp of delta).
 //  * Two records per lane in flight, ping-pong: the load of trip t + 2 is issued as soon as trip t's record has been
@@ -470,7 +473,8 @@ __device__ __forceinline__ void k9_scan_out(const float* __restrict__ prow, int 
     const float e1 = (0.f < side * k1) ? eps : -eps;
     K9Px<MODE> a = k9_load_px<MODE>(p, mine > 0);
     K9Px<MODE> b = k9_load_px<MODE>(p + 32 * FL, mine > 32);
-    for (int t = 64; t < n + 64; t += 64) {   // t = first pixel of the trip pair AFTER the one being evaluated
+    int t = 64;   // first pixel of the trip pair AFTER the one being evaluated
+    for (; t < n; t += 64) {   // every lane of these pairs has a pixel
         p += 64 * FL;
         k9_term<MODE>(a, r0, r1, r2, ra, delta, k0, k1, e0, e1, acc0, acc1);
         a = k9_load_px<MODE>(p, mine > t);
@@ -478,6 +482,9 @@ __device__ __forceinline__ void k9_scan_out(const float* __restrict__ prow, int 
         b = k9_load_px<MODE>(p + 32 * FL, mine > t + 32);
         delta += 64.f;
     }
+    // the last pair (t - 64 < n <= t), peeled so that only it pays for the past-the-end select
+    k9_term<MODE>(a, r0, r1, r2, ra, (mine > t - 64) ? delta : side, k0, k1, e0, e1, acc0, acc1);
+    k9_term<MODE>(b, r0, r1, r2, ra, (mine > t - 32) ? delta + 32.f : side, k0, k1, e0, e1, acc0, acc1);
 }
 
 // One (edge, axis) pass of the reference's per-face loop (:386-410): the edge's vertices in (major, minor) pixel

@@ -30,6 +30,13 @@ def lib():
         L.nmr_oracle_backward_textures.argtypes = [i, f, i, f, f, I, I, I, I]
         L.nmr_oracle_backward_depth_map.restype = None
         L.nmr_oracle_backward_depth_map.argtypes = [f, f, i, f, f, f, f, I, I, I]
+        d = C.POINTER(C.c_double)
+        L.nmr_oracle_backward_pixel_map_stats.restype = None
+        L.nmr_oracle_backward_pixel_map_stats.argtypes = [f, i, f, f, f, f, f, I, I, I, F, I, I, d, d, d, i, i]
+        L.nmr_oracle_backward_textures_stats.restype = None
+        L.nmr_oracle_backward_textures_stats.argtypes = [i, f, i, f, f, I, I, I, I, d, d, i]
+        L.nmr_oracle_backward_depth_map_stats.restype = None
+        L.nmr_oracle_backward_depth_map_stats.argtypes = [f, f, i, f, f, f, f, I, I, I, d, d, i]
         _lib = L
     return _lib
 
@@ -40,6 +47,10 @@ def _f(a):
 
 def _i(a):
     return a.ctypes.data_as(C.POINTER(C.c_int32))
+
+
+def _d(a):
+    return a.ctypes.data_as(C.POINTER(C.c_double))
 
 
 def forward(faces, textures, image_size, near=0.1, far=100.0, eps=1e-4, background_color=(0, 0, 0),
@@ -101,3 +112,47 @@ def backward(faces, textures, fwd, image_size, eps=1e-4, grad_rgb_map=None, grad
                                         _f(np.ascontiguousarray(fwd["face_inv_map"])), _f(fwd["weight_map"]),
                                         _f(g_d), _f(grad_faces), B, nf, H)
     return grad_faces, grad_textures
+
+
+def backward_stats(faces, textures, fwd, image_size, eps=1e-4, grad_rgb_map=None, grad_alpha_map=None,
+                   grad_depth_map=None, return_rgb=True, return_alpha=True, return_depth=True):
+    """backward() plus float64 statistics of every sum, for per-element error bounds (nmr_oracle.c):
+    grad_faces / grad_textures (the float results, as backward() returns them) and
+      k9_g64, k9_T, k9_R, k9_cnt, k9_chain  [B,nf,3,3]  (K9: see k9_stats; zero without rgb / alpha)
+      k10_g64, k10_T, k10_cnt               like textures (K10; None without rgb)
+      k11_g64, k11_T, k11_cnt               [B,nf,3,3]   (K11; zero without depth)"""
+    L = lib()
+    fc = np.ascontiguousarray(faces, np.float32)
+    B, nf = fc.shape[:2]
+    H = int(image_size)
+    z64 = lambda: np.zeros((B, nf, 3, 3), np.float64)
+    z32 = lambda: np.zeros((B, nf, 3, 3), np.int32)
+    out = dict(k9_g64=z64(), k9_T=z64(), k9_R=z64(), k9_cnt=z32(), k9_chain=z32(),
+               k11_g64=z64(), k11_T=z64(), k11_cnt=z32(), k10_g64=None, k10_T=None, k10_cnt=None)
+    grad_faces = np.zeros((B, nf, 3, 3), np.float32)
+    one = np.zeros(1, np.float32)
+    g_rgb = np.ascontiguousarray(grad_rgb_map, np.float32) if return_rgb else one
+    g_a = np.ascontiguousarray(grad_alpha_map, np.float32) if return_alpha else one
+    if return_rgb or return_alpha:
+        L.nmr_oracle_backward_pixel_map_stats(
+            _f(fc), _i(fwd["face_index_map"]), _f(fwd["rgb_map"]) if return_rgb else _f(one),
+            _f(fwd["alpha_map"]) if return_alpha else _f(one), _f(g_rgb), _f(g_a), _f(grad_faces), B, nf, H,
+            np.float32(eps), int(return_rgb), int(return_alpha), _d(out["k9_g64"]), _d(out["k9_T"]), _d(out["k9_R"]),
+            _i(out["k9_cnt"]), _i(out["k9_chain"]))
+    grad_textures = None
+    if return_rgb:
+        tx = np.ascontiguousarray(textures, np.float32)
+        grad_textures = np.zeros_like(tx)
+        out.update(k10_g64=np.zeros(tx.shape, np.float64), k10_T=np.zeros(tx.shape, np.float64),
+                   k10_cnt=np.zeros(tx.shape, np.int32))
+        L.nmr_oracle_backward_textures_stats(_i(fwd["face_index_map"]), _f(fwd["sampling_weight_map"]),
+                                             _i(fwd["sampling_index_map"]), _f(g_rgb), _f(grad_textures), B, nf, H,
+                                             tx.shape[2], _d(out["k10_g64"]), _d(out["k10_T"]), _i(out["k10_cnt"]))
+    if return_depth:
+        g_d = np.ascontiguousarray(grad_depth_map, np.float32)
+        L.nmr_oracle_backward_depth_map_stats(_f(fc), _f(fwd["depth_map"]), _i(fwd["face_index_map"]),
+                                              _f(np.ascontiguousarray(fwd["face_inv_map"])), _f(fwd["weight_map"]),
+                                              _f(g_d), _f(grad_faces), B, nf, H, _d(out["k11_g64"]), _d(out["k11_T"]),
+                                              _i(out["k11_cnt"]))
+    out.update(grad_faces=grad_faces, grad_textures=grad_textures)
+    return out
