@@ -1,5 +1,5 @@
-"""Normal-mapped rendering: port of the reference's demo1.5-SSS.py WITHOUT subsurface scattering (SSS is not ported;
-`with_SSS` is accepted and ignored).  Same settings otherwise: the head at texture_res 15 with its `map_normal` bump map,
+"""Normal-mapped rendering: port of the reference's demo1.5-SSS.py, by default without subsurface scattering; --sss
+renders with it (Lighting's texture-space SSS, lighting.SSS).  Same settings otherwise: the head at texture_res 15 with its `map_normal` bump map,
 SoftRas with dist_func='barycentric' and aggr_func_rgb='hard' at 1024^2, ambient 0.45 and a directional light of 1
 from (0.65, -0.2, -1), look_at camera at distance 2, elevation 20, 90 views every 4 degrees of azimuth.  The surface
 lighting takes the normal-map branch: one normal per texel from normal_textures and the per-face TBN, shaded by the
@@ -8,7 +8,10 @@ fused kernel b200r_normal_mapped_lighting_forward.
 The head (data/head/{head.obj, head.mtl, lambertian.jpg, bump.png}) is used when tools/stage_assets.py has staged it;
 otherwise a generated UV sphere with a procedural 16-bit bump map stands in, and the script says so.
 
-    python examples/demo1_5_render_normal_map.py [-o DIR] [--size 1024] [--step 4] [--fit [--fit-iters 100]]
+    python examples/demo1_5_render_normal_map.py [-o DIR] [--size 1024] [--step 4] [--sss] [--fit [--fit-iters 100]]
+
+--sss lights the mesh with the reference's SSS (with_SSS, as demo1.5-SSS.py builds its head): the irradiance is blurred
+in texture space, modulated by the surface stretch, before it is baked back into the textures.
 
 --fit then recovers the normal map from those renders: it starts from flat tangent-space normals (0, 0, 1), renders
 the same views, and minimises the squared image difference with Adam, through the fused kernel's gradient to the normal
@@ -73,11 +76,12 @@ def load_mesh(device, texture_res=15, sphere_dir=None):
     return mesh, name
 
 
-def render_views(r, mesh, normal_textures, azimuths):
-    """One [3, H, W] image per azimuth, with `normal_textures` in place of the mesh's."""
+def render_views(r, mesh, normal_textures, azimuths, sss=False):
+    """One [3, H, W] image per azimuth, with `normal_textures` in place of the mesh's; sss: with subsurface scattering."""
     out = []
     for azimuth in azimuths:
-        m = jr.Mesh(mesh.vertices, mesh.faces, textures=mesh.textures, normal_textures=normal_textures, TBN=mesh.TBN)
+        m = jr.Mesh(mesh.vertices, mesh.faces, textures=mesh.textures, normal_textures=normal_textures, TBN=mesh.TBN,
+                    with_SSS=sss, face_texcoords=mesh.face_texcoords)
         r.transform.set_eyes_from_angles(CAMERA_DISTANCE, ELEVATION, azimuth)
         out.append(r.render_mesh(m, mode='rgb')[0])
     return out
@@ -116,6 +120,7 @@ def main(argv=None):
     p.add_argument("-o", "--output-dir", default="demo1_5_output")
     p.add_argument("--size", type=int, default=1024)
     p.add_argument("--step", type=int, default=4, help="azimuth step in degrees (4: the reference's 90 views)")
+    p.add_argument("--sss", action="store_true", help="light the frames with subsurface scattering")
     p.add_argument("--fit", action="store_true")
     p.add_argument("--fit-iters", type=int, default=100)
     p.add_argument("--fit-views", type=int, default=8)
@@ -126,11 +131,12 @@ def main(argv=None):
     os.makedirs(a.output_dir, exist_ok=True)
     with tempfile.TemporaryDirectory() as d:
         mesh, name = load_mesh(dev, sphere_dir=d)
-    print("mesh: %s (%d faces, %d texels per face); no SSS" % (name, mesh.faces.shape[1], mesh.textures.shape[2]))
+    print("mesh: %s (%d faces, %d texels per face); %s" % (name, mesh.faces.shape[1], mesh.textures.shape[2],
+                                                         "SSS" if a.sss else "no SSS"))
     r = renderer(a.size)
     with torch.no_grad():
         for k, azimuth in enumerate(range(0, 360, a.step)):
-            img = render_views(r, mesh, mesh.normal_textures, [azimuth])[0]
+            img = render_views(r, mesh, mesh.normal_textures, [azimuth], sss=a.sss)[0]
             frame = (255 * img.permute(1, 2, 0).clamp(0, 1).cpu().numpy()).astype(np.uint8)
             cv2.imwrite(os.path.join(a.output_dir, "rotation_%03d.png" % k), np.ascontiguousarray(frame[:, :, ::-1]))
     print("wrote %d frames to %s" % (len(range(0, 360, a.step)), a.output_dir))

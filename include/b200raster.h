@@ -355,6 +355,29 @@ B200R_API int b200r_vol_resample(const float* z_vals, const float* bins, const f
                                  float* z_samples, float* z_vals_fine, int num_rays, int num_bins, int num_importance,
                                  void* stream);
 
+/* ---- texture-space subsurface scattering ---------------------------------------------------------------------------
+ * Replaces the map stages of SSS (jrender/renderer/lighting/lighting.py:108-150): computeStretchMap
+ * (renderer/utils/ToStretchMap.py:5-13) and the gaussian_blur / _blur_for_SSS ops (renderer/utils/gaussian_blur.py:4-204).
+ * Maps are float32 device planes [H, W], row 0 = the top row of the SoftRas image they were rasterized into; [3, H, W]
+ * inputs are planar (the first three planes of a SoftRas soft_colors [4, H, W] can be passed as they are).  No gradient.
+ *   b200r_sss_stretch: world_map [3, H, W] (world coordinates, before the reference's `* 7`) -> stretch_u, stretch_v
+ *       [H, W]: 1 / |7 (w(y, x) - w(y, x + 1))| and 1 / |7 (w(y, x) - w(y + 1, x))| with the last column / row replicated,
+ *       each clamped to [0, 1].  One launch.
+ *   b200r_sss_blur_pyramid: for each level i < num_levels, stretch_u <- blur_x(stretch_u, mod = stretch_u),
+ *       irr <- blur_x(irr, mod = stretch_u), stretch_v <- blur_y(stretch_v, mod = stretch_v), irr <- blur_y(irr, mod =
+ *       stretch_v), final_c += weights[c * num_levels + i] * irr_c; then final = final * irradiance_map + specular_map,
+ *       written to out_map [H, W, 3] with the rows flipped.  The blurs are the reference kernels' 7-tap modulated blurs
+ *       with taps [num_levels][7] and tap_widths [num_levels] (GaussWidth); taps, tap_widths and weights [3][num_levels]
+ *       are HOST arrays.  irradiance_map and specular_map [3, H, W]; stretch_u / stretch_v are read only.  The maps must be
+ *       square (the reference's y kernel clamps rows against the width); 1 <= num_levels <= 8.  2 * num_levels launches.
+ *       workspace: b200r_sss_workspace_bytes(H, W) bytes (13 maps; 0 for non-positive sizes). */
+B200R_API size_t b200r_sss_workspace_bytes(int height, int width);
+B200R_API int b200r_sss_stretch(const float* world_map, float* stretch_u, float* stretch_v, int height, int width, void* stream);
+B200R_API int b200r_sss_blur_pyramid(const float* stretch_u, const float* stretch_v, const float* irradiance_map,
+                                     const float* specular_map, float* out_map, void* workspace, size_t workspace_bytes,
+                                     const float* taps, const float* tap_widths, const float* weights, int num_levels,
+                                     int height, int width, void* stream);
+
 /* Launch counter: number of kernels this library has launched in this process
  * (bench.py reports the delta over the timed region as "gpu_launches"). */
 B200R_API unsigned long long b200r_launch_count(void);
@@ -378,7 +401,7 @@ enum { B200R_K_FACE_SETUP = 0, B200R_K_COARSE_BIN = 1, B200R_K_SOFTRAS_FWD = 2, 
        B200R_K_PROJECT_FWD = 11, B200R_K_PROJECT_BWD = 12, B200R_K_FLATTEN_LOSS = 13, B200R_K_LAPLACIAN_LOSS = 14,
        B200R_K_LIGHTING = 15, B200R_K_BAKE = 16, B200R_K_ATLAS = 17, B200R_K_VOXEL_SURFACE = 18,
        B200R_K_VOXEL_FILL = 19, B200R_K_CHUNK_RECTS = 20, B200R_K_DEBUG = 21, B200R_K_VOL_COMPOSITE_FWD = 22,
-       B200R_K_VOL_COMPOSITE_BWD = 23, B200R_K_VOL_RESAMPLE = 24, B200R_K_COUNT };
+       B200R_K_VOL_COMPOSITE_BWD = 23, B200R_K_VOL_RESAMPLE = 24, B200R_K_SSS = 25, B200R_K_COUNT };
 B200R_API void b200r_profile_enable(int on);
 B200R_API void b200r_profile_reset(void);
 B200R_API int b200r_profile_read(int kernel, double* total_ms, long long* launches);

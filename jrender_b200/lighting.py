@@ -6,9 +6,13 @@ paths the rasterizer demos use: ambient + directional light in 'surface' and 've
 including the Cook-Torrance specular branch the reference takes by default
 (Mesh.with_specular defaults to True, structures/mesh.py:74).  Normal-mapped meshes (mesh.normal_textures, one normal
 per texel from surface_ResNormals) take the surface branch's normal-map path: one fused kernel forward and one backward
-(b200r_normal_mapped_lighting_*), or the op-by-op directional_lighting_texels.  SSS (with_SSS is accepted and ignored)
-and the Gbuffer debug modes are not mirrored.
+(b200r_normal_mapped_lighting_*), or the op-by-op directional_lighting_texels.  Meshes with with_SSS and SoftRas
+surface textures take the texture-space subsurface scattering of lighting.py:86-156 (SSS below) on both surface
+branches.  The Gbuffer debug modes are not mirrored.
 """
+import ctypes as C
+import math
+
 import torch
 from torch import nn
 import torch.nn.functional as F
@@ -222,6 +226,91 @@ def _normalized_direction(d):
     return F.normalize(t, dim=0, eps=1e-12).tolist()
 
 
+SSS_IMAGE_SIZE = 2048                                             # lighting.py:90
+SSS_TAP_NUM = 7                                                   # :117
+SSS_GAUSSIAN_BASIS = (0, 25, 100, 400)                            # :113: levels of variance 25, 75 and 300
+SSS_WEIGHTS = ((0.7, 0.2, 0.1), (0.1, 0.2, 0.7), (0.1, 0.2, 0.7))  # :123-126, [channel][level]
+
+
+def _sss_taps(v, tap_num=SSS_TAP_NUM):
+    """gaussian_blur.py:7-13: the tap weights Gauss[i] = sqrt(v) N(v; -sqrt(v)(3 - i)) in Python doubles, and GaussWidth
+    = sqrt(v); both are stored as float32 by the caller."""
+    width = math.sqrt(v)
+    g1 = lambda r: math.exp(-r ** 2 / (2 * v)) / math.sqrt(2 * math.pi * v)
+    return [width * g1(-width * ((tap_num - 1) / 2 - i)) for i in range(tap_num)], width
+
+
+def _sss_maps(diffuseLight, specular, mesh):
+    """lighting.py:88-106: the world-coordinate, irradiance and specular maps of SSS, each the [1, 4, S, S] output of
+    one texture-space SoftRas forward (the face UVs as positions); the kernels read their first three planes as the
+    reference's [S, S, 3] maps."""
+    from .softras import SoftRasterizeFunction
+    dev = mesh.textures.device
+    irradiance = torch.sqrt(mesh.textures * diffuseLight)
+    rasterize = SoftRasterizeFunction(image_size=SSS_IMAGE_SIZE, background_color=[0, 0, 0], near=1, far=100, fill_back=True,
+                                      eps=1e-5, sigma_val=1e-5, dist_func='barycentric', dist_eps=1e-5,
+                                      gamma_val=1e-4, aggr_func_rgb='hard', aggr_func_alpha='prod',
+                                      texture_type='surface')
+    # [1, nf, 3, 3] as three texels per face in the reference (:97); its SoftRas samples a surface texture of T texels
+    # at resolution int(sqrt(T)) = 1, i.e. texel 0 (soft_rasterize.py:157-166), so every pixel of a face takes vertex 0's
+    # position and the map is flat over each face.  Passing that texel alone rasterizes the same map.
+    worldcoord_textures = ((mesh.face_vertices + 1) / 2 * 255.)[:, :, :1]
+    coords = (mesh.face_texcoords.to(dev, torch.float32) - 0.5) * 2
+    coords = torch.cat([coords, torch.full(tuple(coords.shape[:3]) + (1,), 1.5, dtype=torch.float32, device=dev)], dim=3)
+    world_map = rasterize(coords, worldcoord_textures)
+    irradiance_map = rasterize(coords, irradiance)
+    specular_map = rasterize(coords, specular)
+    return world_map, irradiance_map, specular_map
+
+
+def SSS(diffuseLight, specular, mesh):
+    """Texture-space subsurface scattering, lighting.py:86-156: the mesh's textures [1, nf, R*R, 3] lit by diffuseLight
+    and specular ([1, nf, 1, 3] per face, or [1, nf, R*R, 3] per texel), returned as new textures [1, nf, R*R, 3]
+    (unclamped; Lighting clamps them).
+
+    sqrt(textures * diffuse), the world coordinates (face_vertices + 1) / 2 * 255 and the specular light are rasterized
+    into the 2048^2 texture space (the face UVs as positions) by the SoftRas forward; b200r_sss_stretch turns the world
+    coordinate map into the clamped stretch maps; b200r_sss_blur_pyramid blurs the irradiance over three levels, modulated
+    by the stretch, and composes `sum_k w_k blur_k * irradiance + specular`; the bake samples that map back into textures.
+
+    As in the reference, gradients stop here: the result does not require grad.  The batch must be 1, the mesh must carry
+    face_texcoords, and its textures must hold texture_res^2 texels per face (ValueError otherwise)."""
+    from . import io
+    tx = mesh.textures
+    if tx.dim() != 4 or tx.shape[0] != 1:
+        raise ValueError("SSS: needs a batch of one mesh with SoftRas surface textures [1, nf, T, 3], got %s"
+                         % (tuple(tx.shape),))
+    ftc = mesh.face_texcoords
+    if ftc is None:
+        raise ValueError("SSS: the mesh has no face_texcoords (load it with Mesh.from_obj(..., load_texture=True))")
+    nf, T, R = tx.shape[1], tx.shape[2], int(mesh.texture_res)
+    if T != R * R:
+        raise ValueError("SSS: %d texels per face, texture_res %d needs %d" % (T, R, R * R))
+    if tuple(ftc.shape) != (1, nf, 3, 2):
+        raise ValueError("SSS: face_texcoords %s do not match %d faces" % (tuple(ftc.shape), nf))
+    dev = tx.device
+    S = SSS_IMAGE_SIZE
+    with torch.no_grad():
+        world_map, irradiance_map, specular_map = _sss_maps(diffuseLight, specular, mesh)
+        stretch_u = torch.empty((S, S), dtype=torch.float32, device=dev)
+        stretch_v = torch.empty_like(stretch_u)
+        _lib.call("b200r_sss_stretch", dev, world_map, stretch_u, stretch_v, S, S)
+        variances = [SSS_GAUSSIAN_BASIS[i + 1] - SSS_GAUSSIAN_BASIS[i] for i in range(len(SSS_GAUSSIAN_BASIS) - 1)]
+        L = len(variances)
+        taps, widths = zip(*[_sss_taps(v) for v in variances])
+        taps = (C.c_float * (L * SSS_TAP_NUM))(*[t for level in taps for t in level])
+        widths = (C.c_float * L)(*widths)
+        weights = (C.c_float * (3 * L))(*[w for channel in SSS_WEIGHTS for w in channel])
+        nbytes = _lib.lib().b200r_sss_workspace_bytes(S, S)
+        workspace = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+        final_map = torch.empty((S, S, 3), dtype=torch.float32, device=dev)
+        _lib.call("b200r_sss_blur_pyramid", dev, stretch_u, stretch_v, irradiance_map, specular_map, final_map, workspace,
+                  nbytes, taps, widths, weights, L, S, S)
+        final = io.bake_textures_for_softras(final_map, ftc[0], torch.ones((nf, R * R, 3), dtype=torch.float32, device=dev),
+                                             torch.ones((nf,), dtype=torch.int32, device=dev), device=dev)
+    return final[None]
+
+
 class AmbientLighting(nn.Module):
     def __init__(self, light_intensity=0.5, light_color=(1, 1, 1)):
         super(AmbientLighting, self).__init__()
@@ -363,9 +452,37 @@ class Lighting(nn.Module):
         mesh.textures = lit
         return mesh
 
+    def _subsurface(self, mesh, eyes):
+        """lighting.py:182-201 with mesh.with_SSS and 4-D textures: the op-by-op diffuse and specular light of either
+        surface branch (per face, or per texel with a normal map), then clamp(SSS(diffuse, specular, mesh), 0, 1)."""
+        if mesh.normal_textures is not None:
+            self._check_normal_map(mesh)
+            diffuseLight = torch.zeros(mesh.textures.shape, dtype=mesh.textures.dtype, device=mesh.vertices.device)
+            specularLight = torch.zeros_like(diffuseLight)
+            diffuseLight = self.ambient(diffuseLight)
+            for d in self.directionals:
+                diffuseLight, specularLight = directional_lighting_texels(
+                    diffuseLight, specularLight, mesh.surface_ResNormals, d.light_intensity, d.light_color,
+                    d.light_direction, torch.sum(mesh.face_vertices, dim=2) / 3.0, eyes, mesh.with_specular,
+                    mesh.metallic_textures, mesh.roughness_textures)
+        else:
+            diffuseLight = torch.zeros(mesh.faces.shape, dtype=torch.float32, device=mesh.vertices.device)
+            specularLight = torch.zeros_like(diffuseLight)
+            diffuseLight = self.ambient(diffuseLight)
+            for directional in self.directionals:
+                diffuseLight, specularLight = directional(
+                    diffuseLight, specularLight, mesh.surface_normals, torch.sum(mesh.face_vertices, dim=2) / 3.0, eyes,
+                    mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
+            diffuseLight = diffuseLight[:, :, None, :]
+            specularLight = specularLight[:, :, None, :]
+        mesh.textures = torch.clamp(SSS(diffuseLight, specularLight, mesh), 0.0, 1.0)
+        return mesh
+
     def forward(self, mesh, eyes=None):
         if self.Gbuffer == "albedo":
             return mesh
+        if self.light_mode == 'surface' and mesh.with_SSS and mesh.textures.dim() == 4:
+            return self._subsurface(mesh, eyes)
         if self.light_mode == 'surface' and mesh.normal_textures is not None:
             return self._normal_mapped(mesh, eyes)
         if self.light_mode == 'surface' and self._fusable(mesh, eyes):

@@ -3,8 +3,8 @@
 Holds vertices [B,nv,3], faces [B,nf,3] and textures; lazily gathers face_vertices
 [B,nf,3,3] / face_textures -- the two tensors the rasterizer consumes.  Only the attributes the
 rasterizer path (Renderer -> Lighting -> Transform -> rasterizer) reads are mirrored, plus export (save_obj), voxelize
-and normal maps (normal_textures, TBN, face_texcoords, surface_ResNormals); SSS is outside the scope (SURVEY.md
-section 8).
+and normal maps (normal_textures, TBN, face_texcoords, surface_ResNormals).  with_SSS makes Lighting take the
+texture-space subsurface scattering (lighting.SSS), which needs face_texcoords and a batch of one.
 """
 import numpy as np
 import torch
