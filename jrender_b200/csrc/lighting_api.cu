@@ -109,13 +109,19 @@ __device__ __forceinline__ float mean_tm(const float* p, int Tm) {   // torch.su
     return s / (float)Tm;
 }
 
-// surface normal the way the mirror forms it: float64 cross product of float32 edge vectors, normalised, back to float32
-__device__ __forceinline__ void normal_f64(const float v[9], float N[3]) {
+// torch.clamp(x, 0, 1): NaN stays NaN (fmaxf alone would return 0 for it)
+__device__ __forceinline__ float clamp01(float x) { return x != x ? x : fminf(fmaxf(x, 0.0f), 1.0f); }
+
+// surface normal the way the mirror forms it: float64 cross product of float32 edge vectors, normalised, back to float32.
+// Returns the unclamped norm |c| (NaN for a non-finite face).
+__device__ __forceinline__ double normal_f64(const float v[9], float N[3]) {
     const double ax = (double)(v[0] - v[3]), ay = (double)(v[1] - v[4]), az = (double)(v[2] - v[5]);   // v10 = v0 - v1
     const double bx = (double)(v[6] - v[3]), by = (double)(v[7] - v[4]), bz = (double)(v[8] - v[5]);   // v12 = v2 - v1
     const double cx = by * az - bz * ay, cy = bz * ax - bx * az, cz = bx * ay - by * ax;               // cross(v12, v10)
-    const double n = fmax(sqrt(cx * cx + cy * cy + cz * cz), 1e-12);
+    const double len = sqrt(cx * cx + cy * cy + cz * cz);
+    const double n = fmax(len, 1e-12);
     N[0] = (float)(cx / n); N[1] = (float)(cy / n); N[2] = (float)(cz / n);
+    return len;
 }
 
 __global__ void __launch_bounds__(128)
@@ -147,7 +153,7 @@ k_surface_lighting_fwd(const float* __restrict__ vertices, const int32_t* __rest
     float* o = out + (size_t)i * T * 3;
     for (int t = 0; t < T; t++)
 #pragma unroll
-        for (int c = 0; c < 3; c++) o[t * 3 + c] = fminf(fmaxf(__ldg(tx + t * 3 + c) * d[c] + 1.0f * s[c], 0.0f), 1.0f);   // lighting.py:199-204
+        for (int c = 0; c < 3; c++) o[t * 3 + c] = clamp01(__ldg(tx + t * 3 + c) * d[c] + 1.0f * s[c]);   // lighting.py:199-204
 }
 
 __global__ void __launch_bounds__(128)
@@ -178,7 +184,7 @@ k_surface_lighting_bwd(const float* __restrict__ vertices, const int32_t* __rest
     const float* ey = spec ? eye + (size_t)(Be == 1 ? 0 : b) * 3 : nullptr;
     // values exactly as the forward formed them (masks of the clamp, d out / d tex)
     float N[3], pos[3], d[3], s[3];
-    normal_f64(v, N);
+    const double len = normal_f64(v, N);
 #pragma unroll
     for (int k = 0; k < 3; k++) pos[k] = ((v[k] + v[3 + k]) + v[6 + k]) / 3.0f;
     face_light<float>(N, pos, Lf, ey, m, r, d, s);
@@ -206,7 +212,7 @@ k_surface_lighting_bwd(const float* __restrict__ vertices, const int32_t* __rest
 #pragma unroll
             for (int c = 0; c < 3; c++) {
                 gm += Gd[c] * dm[c].d[0] + Gs[c] * sm[c].d[0];
-                gr += Gd[c] * dm[c].d[1] + Gs[c] * sm[c].d[1];
+                gr += Gs[c] * sm[c].d[1];   // diffuse does not depend on roughness: no Gd term (a NaN Gd stays out)
             }
             gm = gm / (float)Tm;
             gr = gr / (float)Tm;
@@ -223,8 +229,22 @@ k_surface_lighting_bwd(const float* __restrict__ vertices, const int32_t* __rest
     for (int k = 0; k < 9; k++) dv[k] = dvar<9>(v[k], k);
     D a[3] = {dv[0] - dv[3], dv[1] - dv[4], dv[2] - dv[5]};    // v10
     D bb[3] = {dv[6] - dv[3], dv[7] - dv[4], dv[8] - dv[5]};   // v12
-    D Nd[3] = {bb[1] * a[2] - bb[2] * a[1], bb[2] * a[0] - bb[0] * a[2], bb[0] * a[1] - bb[1] * a[0]};
-    normalize3(Nd, 1e-12f);
+    const D c[3] = {bb[1] * a[2] - bb[2] * a[1], bb[2] * a[0] - bb[0] * a[2], bb[0] * a[1] - bb[1] * a[0]};
+    // The normal's value and norm are the forward's float64 ones: on a sliver the float32 cross product and its norm
+    // cancel, and the derivative would be taken at another normal (and the relu branches chosen there).  Only c's
+    // partials come from the float32 duals; each is a sum of edge components, free of that cancellation.  They pass
+    // through normalize's Jacobian (I - N N^T) / |c|, or I / 1e-12 on its eps path, where the norm is the constant.
+    const float n = (float)fmax(len, 1e-12), inv = 1.f / n;
+    const bool on_eps = !(len > 1e-12);
+    D Nd[3];
+#pragma unroll
+    for (int j = 0; j < 3; j++) Nd[j].v = N[j];
+#pragma unroll
+    for (int k = 0; k < 9; k++) {
+        const float Ndc = on_eps ? 0.f : (N[0] * c[0].d[k] + N[1] * c[1].d[k]) + N[2] * c[2].d[k];
+#pragma unroll
+        for (int j = 0; j < 3; j++) Nd[j].d[k] = (c[j].d[k] - N[j] * Ndc) * inv;
+    }
     D pd[3];
 #pragma unroll
     for (int k = 0; k < 3; k++) pd[k] = ((dv[k] + dv[3 + k]) + dv[6 + k]) / 3.0f;
@@ -290,7 +310,7 @@ k_nm_lighting_fwd(const float* __restrict__ vertices, const int32_t* __restrict_
     face_light<float>(N, pos, Lf, spec ? eye + (size_t)(Be == 1 ? 0 : b) * 3 : nullptr, m, r, d, s);
     const float* tx = textures + (size_t)i * 3;
 #pragma unroll
-    for (int c = 0; c < 3; c++) out[(size_t)i * 3 + c] = fminf(fmaxf(__ldg(tx + c) * d[c] + 1.0f * s[c], 0.0f), 1.0f);
+    for (int c = 0; c < 3; c++) out[(size_t)i * 3 + c] = clamp01(__ldg(tx + c) * d[c] + 1.0f * s[c]);
 }
 
 // One warp per (normal-texture batch, face); lanes stride over the face's texels.  With a batch-1 normal texture the warp
@@ -349,7 +369,7 @@ k_nm_lighting_bwd(const float* __restrict__ vertices, const int32_t* __restrict_
 #pragma unroll
                     for (int c = 0; c < 3; c++) {
                         gm += Gd[c] * dm[c].d[0] + Gs[c] * sm[c].d[0];
-                        gr += Gd[c] * dm[c].d[1] + Gs[c] * sm[c].d[1];
+                        gr += Gs[c] * sm[c].d[1];   // as in the flat kernel: no Gd term
                     }
                 }
                 if (grad_metallic != nullptr) grad_metallic[i] = gm;
