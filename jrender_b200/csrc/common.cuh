@@ -31,6 +31,7 @@ struct __align__(16) FaceRec {
     uint32_t rect_r;   // r0 | r1 << 16 : output rows passing check_border (inclusive, row 0 = top)
     uint32_t flags;    // bit k (k<3): face_obt[k]; bit 3: check_face_frontside;
                        // bit 4+k: midrange(z_k) and a finite inv; bit 7+k: midrange(den_k)
+                       // bits 10-15: reach-cull margin in 1/16 px, 0 = none (k_face_setup reach_margin_q)
     uint32_t face_id;  // index within the batch element
     float inv[9];      // face_inv  (:205-217)
     float v[9];        // x0 y0 z0 x1 y1 z1 x2 y2 z2

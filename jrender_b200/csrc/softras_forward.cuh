@@ -9,7 +9,8 @@
 // their 160-byte records in shared memory 24 at a time (one bulk copy per record), every lane marks the staged faces that
 // cover ITS pixel in a private 24-bit mask, and the lanes then walk their masks in lock-step (lowest bit = lowest face
 // id): each pixel visits its faces in ascending id exactly like the reference's `for (fn = 0; fn < nf; fn++)` (:311),
-// minus the faces check_border would skip.
+// minus the faces check_border would skip and, in euclidean mode, the pairs beyond the face's reach (reach_lane_mask),
+// which the reference's body leaves at its distance threshold.
 //
 // Scheduling: a persistent grid pulls blocks from an atomic queue (head `tile_counter`) ordered by descending cost
 // (number of (pixel, face) pairs per block, computed by k_coarse_bin and bucket-sorted by k_tile_order): blocks at
@@ -34,7 +35,7 @@ static_assert(B200R_BLOCK_W * B200R_BLOCK_H == kFwdLanes, "one lane per pixel of
 
 // resident one-warp CTAs per SM the register allocation must allow (96 registers).  H100, C3: forward 1.08 ms at 20, 1.10
 // at 16, 1.29 at 24 (16-record rounds, LDG staging); with bulk copies 1.017 at 20, 1.016 at 22, 1.017 at 18.  Spills
-// (ptxas, sm_90a): the C3 instantiation <2,1,false> 64 B stored / 72 B loaded at 96 registers; the others 0-8 B
+// (ptxas, sm_90a): the C3 instantiation <2,1,false> 60 B stored / 64 B loaded at 96 registers; the others 0-44 B
 constexpr int kFwdMinBlocks = 20;
 
 // ---- mbarrier / bulk-copy (TMA) helpers.  Records are staged by cp.async.bulk + mbarrier rather than LDG -> registers
@@ -249,6 +250,57 @@ __device__ __forceinline__ uint32_t rect_lane_mask(uint32_t rx, uint32_t rr, int
     return (cols * 0x01010101u) & rows;
 }
 
+// Euclidean mode: the lanes a staged record can still shade, i.e. the pixels inside its reach polygon, the rectangle cut
+// by the three edge lines moved out by R: support lines of "triangle + disk(R)" (DESIGN.md §4.4).  Only for records
+// whose k_face_setup margin (flags bits 10-15, 1/16 px) is set.  Local frame: pixels, column / row offsets from the
+// block's first pixel (xb, yb), hs = is / 2; reach = the cull radius without the margin, slack included.  A line's
+// direction need not be exact: its offset is the maximum over the three vertices along the computed direction, so it
+// contains triangle + disk(R) whatever the direction's rounding.  Per block row a line bounds the column range from
+// one side (c <= q or c >= q, q linear in the row); lines too close to horizontal (|a| < 2^-20), or NaN, bound nothing.
+// (The three vertex bisectors as well cut 2 % more pairs than the edges alone and cost more than they save.)
+__device__ __forceinline__ uint32_t reach_lane_mask(const FaceRec& rec, float xb, float yb, float hs, float reach) {
+    const float R = reach + (float)((rec.flags >> 10) & 63u) * 0.0625f;
+    float X[3], Y[3], ux[3], uy[3];
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        X[k] = (rec.v[3 * k] - xb) * hs;
+        Y[k] = (yb - rec.v[3 * k + 1]) * hs;
+    }
+#pragma unroll
+    for (int k = 0; k < 3; k++) {   // unit vector of edge k: v_k -> v_(k+1)
+        const int k1 = (k + 1) % 3;
+        const float ex = X[k1] - X[k], ey = Y[k1] - Y[k];
+        const float rl = rsqrtf(__fmaf_rn(ex, ex, ey * ey));
+        ux[k] = ex * rl;
+        uy[k] = ey * rl;
+    }
+    const float o = __fmaf_rn(ux[0], uy[1], -uy[0] * ux[1]) > 0.f ? 1.f : -1.f;   // (o uy, -o ux) points outward
+    float lo[4] = {0.f, 0.f, 0.f, 0.f}, hi[4] = {7.f, 7.f, 7.f, 7.f};
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        // edge k's outward normal, of length 1 within 2^-21 (the slack in reach covers R's share of that)
+        const float a = o * uy[k], b = -o * ux[k];
+        const float H = fmaxf(fmaxf(__fmaf_rn(a, X[0], b * Y[0]), __fmaf_rn(a, X[1], b * Y[1])), __fmaf_rn(a, X[2], b * Y[2])) + R;
+        const float ra = __fdividef(1.f, a);
+        const float q0 = H * ra, dq = -b * ra;   // row r: a c <= H - b r  <=>  c <= (a > 0) or >= (a < 0) q0 + r dq
+        const bool use = fabsf(a) >= 0x1p-20f;
+        const float h0 = (use && a > 0.f) ? q0 : 7.f, hd = (use && a > 0.f) ? dq : 0.f;
+        const float l0 = (use && a < 0.f) ? q0 : 0.f, ld = (use && a < 0.f) ? dq : 0.f;
+#pragma unroll
+        for (int r = 0; r < 4; r++) {
+            hi[r] = fminf(hi[r], __fmaf_rn((float)r, hd, h0));
+            lo[r] = fmaxf(lo[r], __fmaf_rn((float)r, ld, l0));
+        }
+    }
+    uint32_t m = 0u;
+#pragma unroll
+    for (int r = 0; r < 4; r++) {
+        const int c0 = __float2int_ru(lo[r]), c1 = __float2int_rd(hi[r]);   // 0 <= c0, c1 <= 7
+        if (c0 <= c1) m |= ((2u << c1) - (1u << c0)) << (8 * r);
+    }
+    return m;
+}
+
 // :425-455: a pixel's six output values from its final state.  The three colour quotients share one refined reciprocal
 // (fast_div returns the correctly rounded quotient for every input, exact_math.cuh).
 template <int RGB>
@@ -291,6 +343,11 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
     const int is = P.is, nf = P.nf, K = P.K;
     const int lx = lane & 7, ly = lane >> 3;   // lane = row-major pixel index inside the block = index of the [K][4][8] id planes
     const float threshold = P.dist_eps * P.sigma;  // :289
+    // reach polygon radius in pixels before a face's margin: border (1 + 2^-19) -- border = sqrt(threshold) as
+    // k_face_setup's rectangle uses it -- plus the slack that covers reach_lane_mask's float evaluation (DESIGN.md §4.4).
+    // Radii beyond the image size cull nothing the rectangle does not, and keep that evaluation's magnitudes bounded.
+    float reach = sqrtf(threshold) * (0.5f * (float)is) * (1.f + 0x1p-19f) + (float)(is + 64) * 0x1p-16f;
+    if (!(reach <= (float)is)) reach = -1.f;   // off
     const size_t npix = (size_t)is * is;
     DivConst dc;
     dc.init(P);
@@ -423,8 +480,14 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
                 // ---- per-lane face masks by transposition: lane j turns record j's rectangle, clipped to the 8x4
                 // block, into the 32-bit set of covered lanes; every lane then picks its own bit out of the kFwdChunk
                 // words (kFwdChunk / 4 broadcast LDS.128).
+                // Euclidean mode ANDs in the record's reach polygon when k_face_setup gave it a margin.
                 uint32_t lm = 0u;
-                if (lane < m) lm = rect_lane_mask(S.rec[lane].r.rect_x, S.rec[lane].r.rect_r, tx0, tr0);
+                const float xb = __shfl_sync(FULL, xp, 0), yb = __shfl_sync(FULL, yp, 0);   // the block's first pixel
+                if (lane < m) {
+                    const FaceRec& rec = S.rec[lane].r;
+                    lm = rect_lane_mask(rec.rect_x, rec.rect_r, tx0, tr0);
+                    if (DIST == 2 && reach >= 0.f && (rec.flags >> 10) != 0u) lm &= reach_lane_mask(rec, xb, yb, 0.5f * (float)is, reach);
+                }
                 if (lane < CHUNK) S.lmask[lane] = lm;
                 __syncwarp();
                 unsigned mask = 0u;   // bit j: staged record j covers this lane's pixel (ascending record = ascending face id)

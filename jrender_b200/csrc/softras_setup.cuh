@@ -26,6 +26,61 @@ __device__ __forceinline__ int last_not_above(float lim, int is) {
     return i;
 }
 
+// Reach-cull margin of one face (DESIGN.md §4.4), in 1/16 pixel, 1..63; 0 = the face keeps the rectangle mask.  For
+// every pixel centre p of the face's rectangle [xlo, xhi] x [ylo, yhi] whose distance to the triangle is at least
+// border (1 + 4u) + margin, the euclidean per-pair body computes sign < 0 and dis >= threshold, whichever edge it picks.
+// inv = the record's float inverse, exactly as the body uses it: lam_k(p) = inv_k . (x, y, 1) is affine in p, so its
+// excursion from the true barycentrics (E, S below) is bounded over the rectangle by its four corners, in double.
+__device__ __forceinline__ uint32_t reach_margin_q(const float f[9], const float inv[9], double xlo, double xhi, double ylo,
+                                                  double yhi, int is) {
+    const double u = 0x1p-24, g3 = 3 * u / (1 - 3 * u), g4 = 4 * u / (1 - 4 * u);
+    double M = 0.0, Lmax2 = 0.0;
+    for (int k = 0; k < 3; k++) {
+        if (!isfinite(f[3 * k]) || !isfinite(f[3 * k + 1])) return 0u;
+        M = fmax(M, fmax(fabs((double)f[3 * k]), fabs((double)f[3 * k + 1])));
+        const int k1 = (k + 1) % 3;
+        const double dx = (double)f[3 * k1] - f[3 * k], dy = (double)f[3 * k1 + 1] - f[3 * k + 1];
+        Lmax2 = fmax(Lmax2, dx * dx + dy * dy);
+    }
+    for (int k = 0; k < 9; k++)
+        if (!isfinite(inv[k])) return 0u;
+    const double D = ((double)f[3] - f[0]) * ((double)f[7] - f[1]) - ((double)f[4] - f[1]) * ((double)f[6] - f[0]);
+    // bounded vertices; conditioning: twice the area against the longest edge squared (smallest altitude / longest
+    // edge >= 2^-12) keeps the barycentrics over the rectangle, and with them the rounding terms below, bounded
+    if (!(M <= 4.0) || !(fabs(D) >= 0x1p-12 * Lmax2) || !(Lmax2 > 0.0)) return 0u;
+    const double X = fmax(fabs(xlo), fabs(xhi)), Y = fmax(fabs(ylo), fabs(yhi));
+    double ex = 0.0, ey = 0.0, es = 0.0, lam_max[3] = {0.0, 0.0, 0.0}, mag = 0.0;
+    for (int c = 0; c < 4; c++) {
+        const double px = (c & 1) ? xhi : xlo, py = (c & 2) ? yhi : ylo;
+        double sx = -px, sy = -py, ss = -1.0;
+        for (int k = 0; k < 3; k++) {
+            const double l = (double)inv[3 * k] * px + (double)inv[3 * k + 1] * py + inv[3 * k + 2];
+            sx += l * f[3 * k];
+            sy += l * f[3 * k + 1];
+            ss += l;
+            lam_max[k] = fmax(lam_max[k], fabs(l));
+        }
+        ex = fmax(ex, fabs(sx)); ey = fmax(ey, fabs(sy)); es = fmax(es, fabs(ss));
+    }
+    double sig = 0.0, sig_v = 0.0, W = 0.0;   // sig: the float evaluation of w_k = inv_k . (x, y, 1), summed over k
+    for (int k = 0; k < 3; k++) {
+        const double s = g3 * (fabs((double)inv[3 * k]) * X + fabs((double)inv[3 * k + 1]) * Y + fabs((double)inv[3 * k + 2]));
+        sig += s;
+        sig_v += s * sqrt((double)f[3 * k] * f[3 * k] + (double)f[3 * k + 1] * f[3 * k + 1]);
+        W += lam_max[k] + s;
+        mag += fabs((double)inv[3 * k]) * X + fabs((double)inv[3 * k + 1]) * Y + fabs((double)inv[3 * k + 2]);
+    }
+    const double slop = 0x1p-40 * (mag + 1.0) * (M + X + Y + 1.0);   // the double evaluation above
+    const double E = sqrt(ex * ex + ey * ey) + slop, S = es + sig + slop;
+    if (!(S < 0.5)) return 0u;
+    // (a) all three w in (0, 1): the point sum w_k v_k / sum w_k lies in the triangle and within dA of p
+    const double dA = (sqrt(X * X + Y * Y) * S + E + sig_v) / (1.0 - S);
+    // (b) some w outside (0, 1): the computed (dis_x, dis_y) is p's offset to a point of the triangle, up to dB
+    const double dB = sqrt(2.0) * u * M + E + sig_v + sqrt(2.0) * g4 * (1.0 + u + W) * M;
+    const double q = ceil(fmax(dA, dB) * 0.5 * is * 16.0);
+    return q <= 63.0 ? (uint32_t)fmax(q, 1.0) : 0u;
+}
+
 // One thread per (batch, face).  Computes the 160-byte record, the exact pixel rectangle
 // equivalent to check_border, and (optionally) the reference's faces_info[27].
 // Reference: forward_soft_rasterize_inv_cuda_kernel, cuda/soft_rasterize.py:176-236.
@@ -88,7 +143,6 @@ static __global__ void __launch_bounds__(256) k_face_setup(const float* __restri
         if (midrange(z) && inv_finite) flags |= 16u << k;
         if (midrange(den)) flags |= 128u << k;
     }
-    r.flags = flags;
     r.face_id = (uint32_t)(i % nf);
 #pragma unroll
     for (int k = 0; k < 3; k++) r.col[k] = (T == 1 && tex_type == 0) ? __ldg(textures + (size_t)i * 3 + k) : 0.f;
@@ -102,6 +156,10 @@ static __global__ void __launch_bounds__(256) k_face_setup(const float* __restri
     const int y0 = first_not_below(ylo, is), y1 = last_not_above(yhi, is);
     int r0 = is - 1 - y1, r1 = is - 1 - y0;  // row = is-1-yi (:280)
     if (x0 > x1 || r0 > r1) { x0 = 1; x1 = 0; r0 = 1; r1 = 0; }
+    else if ((flags & 0x3f0u) == 0x3f0u)   // reach-cull margin, bits 10-15 (the forward's euclidean lane masks)
+        flags |= reach_margin_q(f, r.inv, b200r_pix_coord(x0, is), b200r_pix_coord(x1, is), b200r_pix_coord(is - 1 - r1, is),
+                                b200r_pix_coord(is - 1 - r0, is), is) << 10;
+    r.flags = flags;
     r.rect_x = (uint32_t)x0 | ((uint32_t)x1 << 16);
     r.rect_r = (uint32_t)r0 | ((uint32_t)r1 << 16);
 
