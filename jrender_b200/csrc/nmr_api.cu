@@ -9,6 +9,11 @@
 
 using namespace b200r;
 
+// K9's two kernels and its packed record width (floats) per MODE (1: rgb, 2: alpha, 3: both)
+struct K9Kernels { decltype(&k_nmr_pack<1>) pack; decltype(&k_nmr_backward_pixel_map<1>) pixel_map; size_t fl; };
+template <int MODE>
+static constexpr K9Kernels kK9 = {&k_nmr_pack<MODE>, &k_nmr_backward_pixel_map<MODE>, K9Rec<MODE>::FL};
+
 extern "C" {
 
 size_t b200r_nmr_workspace_bytes(int batch_size, int num_faces, int image_size) {
@@ -80,17 +85,15 @@ int b200r_nmr_backward(const float* faces, const int32_t* face_index_map, const 
         if (!scratch || scratch_bytes < need)
             return b200r_fail(B200R_EWORKSPACE, "b200r_nmr_backward: scratch %zu < required %zu bytes", scratch_bytes, need);
         const int mode = (return_rgb ? 1 : 0) | (return_alpha ? 2 : 0);
-        const size_t fl = mode == 1 ? 4 : (mode == 2 ? 2 : 8);   // floats per packed record (K9Rec<MODE>::FL)
+        const K9Kernels k9 = mode == 1 ? kK9<1> : mode == 2 ? kK9<2> : kK9<3>;
         float* ph = reinterpret_cast<float*>(scratch);
-        float* pv = ph + (size_t)B * is * is * fl;
+        float* pv = ph + (size_t)B * is * is * k9.fl;
         const long warps = (long)B * nf;
-        auto pack = mode == 3 ? &k_nmr_pack<3> : mode == 1 ? &k_nmr_pack<1> : &k_nmr_pack<2>;
-        auto pixel_map = mode == 3 ? &k_nmr_backward_pixel_map<3> : mode == 1 ? &k_nmr_backward_pixel_map<1> : &k_nmr_backward_pixel_map<2>;
-        if (int rc = b200r_launch("k_nmr_pack", B200R_K_NMR_PACK, pack, dim3((is + 31) / 32, (is + 31) / 32, B), 256, 0, st, rgb_map,
-                                  alpha_map, grad_rgb_map, grad_alpha_map, ph, pv, is))
+        if (int rc = b200r_launch("k_nmr_pack", B200R_K_NMR_PACK, k9.pack, dim3((is + 31) / 32, (is + 31) / 32, B), 256, 0, st,
+                                  rgb_map, alpha_map, grad_rgb_map, grad_alpha_map, ph, pv, is))
             return rc;
-        if (int rc = b200r_launch("k_nmr_backward_pixel_map", B200R_K_NMR_BWD_PIXEL, pixel_map, (unsigned)((warps + 7) / 8), 256, 0,
-                                  st, faces, face_index_map, rgb_map, alpha_map, ph, pv, grad_faces, B, nf, is, eps))
+        if (int rc = b200r_launch("k_nmr_backward_pixel_map", B200R_K_NMR_BWD_PIXEL, k9.pixel_map, (unsigned)((warps + 7) / 8), 256,
+                                  0, st, faces, face_index_map, rgb_map, alpha_map, ph, pv, grad_faces, B, nf, is, eps))
             return rc;
     }
     if (!return_rgb && !return_depth) return 0;

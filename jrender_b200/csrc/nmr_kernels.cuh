@@ -344,85 +344,8 @@ __device__ __forceinline__ int k9_sel6(int i, const int v[7]) {
     return i == 0 ? v[0] : (i == 1 ? v[1] : (i == 2 ? v[2] : (i == 3 ? v[3] : (i == 4 ? v[4] : v[5]))));
 }
 
-// One line scan of K9 (:486-520 outwards / :556-601 inwards): lanes take consecutive pixels d1_from + lane, + 32, ...
-// of the packed row `prow` (k_nmr_pack) and add their  -diff_grad / dist  terms to acc0 / acc1.
-//   OWNER  inward scan: only pixels whose face_index_map entry is this face count (:573)
-//   BOTH   both vertex terms present (p[1][0] != d0 and p[0][0] != d0, :508/:513): the common, branch-free flavour
-// The loop is the whole cost of the kernel (the outward scan runs to the image border for every edge sample), so it
-// is kept to one record load and ~20 arithmetic instructions per 32 pixels: pointers and the pixel coordinate
-// advance by constants, the `diff_grad <= 0` skip is a select (a NaN still propagates like the reference's
-// `continue` would let it), products are fused (sums of ~10^2..10^3 terms, compared at 2e-5 relative).
-// ref = (r, g, b, alpha) of the sample's in-pixel (outward scan) / out-pixel (inward scan).
-template <int MODE, bool OWNER, bool BOTH>
-__device__ __forceinline__ void k9_scan(const float* __restrict__ prow, const int* __restrict__ fim, int fim_stride,
-                                        int d1_from, int d1_to, int lane, int fn, float r0, float r1, float r2, float ra,
-                                        float d1_cross, float k0, float k1, bool has0, bool has1, float eps,
-                                        float& acc0, float& acc1) {
-    constexpr int FL = K9Rec<MODE>::FL;
-    // offsets inside one image fit 32 bits (is <= 4096: is^2 * FL <= 2^27)
-    const float* __restrict__ p = prow + (d1_from + lane) * FL;
-    const int* __restrict__ o = OWNER ? fim + (d1_from + lane) * fim_stride : nullptr;
-    float d1f = (float)(d1_from + lane);   // exact below 2^24
-    int left = d1_to - d1_from - lane;
-    // software pipeline: the record (and owner) of trip t + 1 is requested before trip t is evaluated -- one trip's
-    // arithmetic is far shorter than an L1 / L2 round trip, and the scan is a chain of dependent trips otherwise
-    float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
-    float ga = 0.f;
-    int own = fn;
-    if (left >= 0) {
-        if (MODE == 2) { const float2 t = __ldg(reinterpret_cast<const float2*>(p)); q.x = t.x; q.y = t.y; }
-        else q = __ldg(reinterpret_cast<const float4*>(p));
-        if (MODE == 3) ga = __ldg(p + 4);
-        if (OWNER) own = __ldg(o);
-    }
-    while (left >= 0) {
-        const float4 c = q;
-        const float cga = ga;
-        const int cown = own;
-        left -= 32;
-        p += 32 * FL;
-        if (OWNER) o += 32 * fim_stride;   // (pointer arithmetic in 64 bits, the product in 32)
-        if (left >= 0) {
-            if (MODE == 2) { const float2 t = __ldg(reinterpret_cast<const float2*>(p)); q.x = t.x; q.y = t.y; }
-            else q = __ldg(reinterpret_cast<const float4*>(p));
-            if (MODE == 3) ga = __ldg(p + 4);
-            if (OWNER) own = __ldg(o);
-        }
-        float diff;
-        if (MODE == 1) diff = __fmaf_rn(-r2, c.w, __fmaf_rn(-r1, c.z, __fmaf_rn(-r0, c.y, c.x)));
-        else if (MODE == 2) diff = __fmaf_rn(-ra, c.y, c.x);
-        else diff = __fmaf_rn(-ra, cga, __fmaf_rn(-r2, c.w, __fmaf_rn(-r1, c.z, __fmaf_rn(-r0, c.y, c.x))));
-        const bool mine = !OWNER || cown == fn;
-        const float d = (mine && !(diff <= 0.f)) ? diff : 0.f;   // :503 / :587 `if (diff_grad <= 0) continue`
-        const float delta = d1f - d1_cross;   // (d1 - d1_cross), one rounding like the reference's
-        d1f += 32.f;
-        if (BOTH || has0) {
-            float dist = delta * k0;
-            dist = (0.f < dist) ? dist + eps : dist - eps;      // :510
-            acc0 = __fmaf_rn(-d, rcp_approx(dist), acc0);
-        }
-        if (BOTH || has1) {
-            float dist = delta * k1;
-            dist = (0.f < dist) ? dist + eps : dist - eps;      // :515
-            acc1 = __fmaf_rn(-d, rcp_approx(dist), acc1);
-        }
-    }
-}
-
-// The outward scan (:486-520), specialised: it is 2/3 of K9's instructions and all of its load latency.
-//  * Every pixel of an outward scan lies strictly beyond the crossing point (d1_out = floor(d1_cross) + 1 or
-//    ceil(d1_cross) - 1, then away from it), so delta = d1 - d1_cross has ONE sign for the whole scan and the reference's
-//    per-pixel `dist = (0 < dist) ? dist + eps : dist - eps` (:510/:515) adds a per-scan constant: dist = fma(delta, k, +-eps)
-//    (|k| >= 2 / is, so delta * k never underflows; no cancellation, so |dist| >= eps).
-//  * Lanes past the end of the scan (only in the last trip pair) evaluate a zero record with delta replaced by `side`
-//    (d1_from - d1_cross), so their dist is nonzero and they add exactly 0.  Their own delta would not do: in a scan toward pixel 0 they sit at d1_in
-//    and beyond, across the crossing, where fma(delta, k, e) can cancel to exactly 0 -- and 0 * inf is NaN.
-//  * `diff_grad <= 0 -> continue` (:503) is max.NaN(diff, 0): a NaN still propagates like the reference's test lets it.
-//  * delta advances by 64 per trip instead of being re-formed from the pixel number (<= 1 ulp of delta).
-//  * Two records per lane in flight, ping-pong: the load of trip t + 2 is issued as soon as trip t's record has been
-//    consumed and is only needed after trip t + 1's arithmetic -- the generic loop below re-used the record's registers
-//    and waited for every load (long-scoreboard stalls dominated).
-// Trip count is warp-uniform; only the loads are predicated.
+// One packed record of k_nmr_pack as every scan holds it: q = (A, gr, gg, gb) for rgb, (A, ga, -, -) for alpha,
+// (A, gr, gg, gb) and ga for both.  Lanes without a pixel (`on` false) get a zero record.
 template <int MODE>
 struct K9Px { float4 q; float ga; };
 
@@ -439,6 +362,92 @@ __device__ __forceinline__ K9Px<MODE> k9_load_px(const float* __restrict__ p, bo
     return r;
 }
 
+// diff_grad = A - sum_k ref_k * grad_k as one fma chain off A (the negations are operand modifiers): one instruction
+// fewer per record than forming the sum first.  ref = (r, g, b, alpha) of the sample's in-pixel (outward scan) /
+// out-pixel (inward scan).
+template <int MODE>
+__device__ __forceinline__ float k9_diff(const K9Px<MODE>& c, float r0, float r1, float r2, float ra) {
+    if (MODE == 1) return __fmaf_rn(-r2, c.q.w, __fmaf_rn(-r1, c.q.z, __fmaf_rn(-r0, c.q.y, c.q.x)));
+    if (MODE == 2) return __fmaf_rn(-ra, c.q.y, c.q.x);
+    return __fmaf_rn(-ra, c.ga, __fmaf_rn(-r2, c.q.w, __fmaf_rn(-r1, c.q.z, __fmaf_rn(-r0, c.q.y, c.q.x))));
+}
+
+// acc += -d / dist with the reference's per-pixel distance  dist = delta * k + (dist > 0 ? eps : -eps)  (:510/:515)
+__device__ __forceinline__ void k9_guarded_term(float d, float delta, float k, float eps, float& acc) {
+    float dist = delta * k;
+    dist = (0.f < dist) ? dist + eps : dist - eps;
+    acc = __fmaf_rn(-d, rcp_approx(dist), acc);
+}
+
+// Adds a pass's two running sums to the face's six gradient slots gacc[vertex * 2 + (0: x, 1: y)]: acc0 / acc1 belong
+// to vertex pi0 / pi1 of the pass's edge, coordinate (1 - axis).  Compare-and-add keeps gacc in registers.
+__device__ __forceinline__ void k9_add_slots(int pass, float acc0, float acc1, float gacc[6]) {
+    const int edge = pass >> 1, axis = pass & 1;
+    const int g0 = edge * 2 + (1 - axis), g1 = ((edge == 2) ? 0 : edge + 1) * 2 + (1 - axis);
+#pragma unroll
+    for (int k = 0; k < 6; k++) {
+        if (k == g0) gacc[k] += acc0;
+        if (k == g1) gacc[k] += acc1;
+    }
+}
+
+// One line scan of K9 (:486-520 outwards / :556-601 inwards): lanes take consecutive pixels d1_from + lane, + 32, ...
+// of the packed row `prow` (k_nmr_pack) and add their  -diff_grad / dist  terms to acc0 / acc1 (only the terms whose
+// vertex is off the sample's line: has0 = p[1][0] != d0, has1 = p[0][0] != d0, :508/:513).
+//   OWNER  inward scan: only pixels whose face_index_map entry is this face count (:573)
+// The loop is kept to one record load and ~20 arithmetic instructions per 32 pixels: pointers and the pixel
+// coordinate advance by constants, the `diff_grad <= 0` skip is a select (a NaN still propagates like the reference's
+// `continue` would let it), products are fused (sums of ~10^2..10^3 terms, compared at 2e-5 relative).
+template <int MODE, bool OWNER>
+__device__ __forceinline__ void k9_scan(const float* __restrict__ prow, const int* __restrict__ fim, int fim_stride,
+                                        int d1_from, int d1_to, int lane, int fn, float r0, float r1, float r2, float ra,
+                                        float d1_cross, float k0, float k1, bool has0, bool has1, float eps,
+                                        float& acc0, float& acc1) {
+    constexpr int FL = K9Rec<MODE>::FL;
+    // offsets inside one image fit 32 bits (is <= 4096: is^2 * FL <= 2^27)
+    const float* __restrict__ p = prow + (d1_from + lane) * FL;
+    const int* __restrict__ o = OWNER ? fim + (d1_from + lane) * fim_stride : nullptr;
+    float d1f = (float)(d1_from + lane);   // exact below 2^24
+    int left = d1_to - d1_from - lane;
+    // software pipeline: the record (and owner) of trip t + 1 is requested before trip t is evaluated -- one trip's
+    // arithmetic is far shorter than an L1 / L2 round trip, and the scan is a chain of dependent trips otherwise
+    K9Px<MODE> q = k9_load_px<MODE>(p, left >= 0);
+    int own = fn;
+    if (OWNER && left >= 0) own = __ldg(o);
+    while (left >= 0) {
+        const K9Px<MODE> c = q;
+        const int cown = own;
+        left -= 32;
+        p += 32 * FL;
+        if (OWNER) o += 32 * fim_stride;   // (pointer arithmetic in 64 bits, the product in 32)
+        if (left >= 0) {
+            q = k9_load_px<MODE>(p, true);
+            if (OWNER) own = __ldg(o);
+        }
+        const float diff = k9_diff<MODE>(c, r0, r1, r2, ra);
+        const bool mine = !OWNER || cown == fn;
+        const float d = (mine && !(diff <= 0.f)) ? diff : 0.f;   // :503 / :587 `if (diff_grad <= 0) continue`
+        const float delta = d1f - d1_cross;   // (d1 - d1_cross), one rounding like the reference's
+        d1f += 32.f;
+        if (has0) k9_guarded_term(d, delta, k0, eps, acc0);
+        if (has1) k9_guarded_term(d, delta, k1, eps, acc1);
+    }
+}
+
+// The outward scan (:486-520), specialised: it is 2/3 of K9's instructions and all of its load latency.
+//  * Every pixel of an outward scan lies strictly beyond the crossing point (d1_out = floor(d1_cross) + 1 or
+//    ceil(d1_cross) - 1, then away from it), so delta = d1 - d1_cross has ONE sign for the whole scan and the reference's
+//    per-pixel `dist = (0 < dist) ? dist + eps : dist - eps` (:510/:515) adds a per-scan constant: dist = fma(delta, k, +-eps)
+//    (|k| >= 2 / is, so delta * k never underflows; no cancellation, so |dist| >= eps).
+//  * Lanes past the end of the scan (only in the last trip pair) evaluate a zero record with delta replaced by `side`
+//    (d1_from - d1_cross), so their dist is nonzero and they add exactly 0.  Their own delta would not do: in a scan toward pixel 0 they sit at d1_in
+//    and beyond, across the crossing, where fma(delta, k, e) can cancel to exactly 0 -- and 0 * inf is NaN.
+//  * `diff_grad <= 0 -> continue` (:503) is max.NaN(diff, 0): a NaN still propagates like the reference's test lets it.
+//  * delta advances by 64 per trip instead of being re-formed from the pixel number (<= 1 ulp of delta).
+//  * Two records per lane in flight, ping-pong: the load of trip t + 2 is issued as soon as trip t's record has been
+//    consumed and is only needed after trip t + 1's arithmetic -- k9_scan's one-deep pipeline re-uses the record's
+//    registers and, on these scans, waited for every load (long-scoreboard stalls dominated).
+// Trip count is warp-uniform; only the loads are predicated.
 __device__ __forceinline__ float max_nan(float a, float b) {
     float r;
     asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
@@ -448,13 +457,7 @@ __device__ __forceinline__ float max_nan(float a, float b) {
 template <int MODE>
 __device__ __forceinline__ void k9_term(const K9Px<MODE>& c, float r0, float r1, float r2, float ra, float delta,
                                         float k0, float k1, float e0, float e1, float& acc0, float& acc1) {
-    float diff;
-    // A - sum_k ref_k * grad_k as one fma chain off A (the negations are operand modifiers): one instruction fewer per
-    // record than forming the sum first
-    if (MODE == 1) diff = __fmaf_rn(-r2, c.q.w, __fmaf_rn(-r1, c.q.z, __fmaf_rn(-r0, c.q.y, c.q.x)));
-    else if (MODE == 2) diff = __fmaf_rn(-ra, c.q.y, c.q.x);
-    else diff = __fmaf_rn(-ra, c.ga, __fmaf_rn(-r2, c.q.w, __fmaf_rn(-r1, c.q.z, __fmaf_rn(-r0, c.q.y, c.q.x))));
-    const float d = max_nan(diff, 0.f);
+    const float d = max_nan(k9_diff<MODE>(c, r0, r1, r2, ra), 0.f);
     acc0 = __fmaf_rn(-d, rcp_approx(__fmaf_rn(delta, k0, e0)), acc0);
     acc1 = __fmaf_rn(-d, rcp_approx(__fmaf_rn(delta, k1, e1)), acc1);
 }
@@ -621,38 +624,13 @@ k_nmr_backward_pixel_map(const float* __restrict__ faces, const int* __restrict_
             float a0 = 0.f, a1 = 0.f;
             for (int d1 = in_from; d1 <= in_to; d1++) {
                 if (__ldg(fim_img + fim_base + d1 * fim_stride) != fn) continue;   // :573
-                float diff;
-                const float* pr = prow_l + d1 * FL;
-                if (MODE == 1) {
-                    const float4 r4 = __ldg(reinterpret_cast<const float4*>(pr));
-                    diff = r4.x - __fmaf_rn(o2, r4.w, __fmaf_rn(o1, r4.z, o0 * r4.y));
-                } else if (MODE == 2) {
-                    const float2 r2 = __ldg(reinterpret_cast<const float2*>(pr));
-                    diff = r2.x - oa * r2.y;
-                } else {
-                    const float4 r4 = __ldg(reinterpret_cast<const float4*>(pr));
-                    diff = r4.x - __fmaf_rn(oa, __ldg(pr + 4), __fmaf_rn(o2, r4.w, __fmaf_rn(o1, r4.z, o0 * r4.y)));
-                }
+                const float diff = k9_diff<MODE>(k9_load_px<MODE>(prow_l + d1 * FL, true), o0, o1, o2, oa);
                 if (diff <= 0.f) continue;                                          // :587
                 const float delta = (float)d1 - d1_cross;
-                if (has0) {
-                    float dist = delta * k0;
-                    dist = (0.f < dist) ? dist + eps : dist - eps;
-                    a0 = __fmaf_rn(-diff, rcp_approx(dist), a0);
-                }
-                if (has1) {
-                    float dist = delta * k1;
-                    dist = (0.f < dist) ? dist + eps : dist - eps;
-                    a1 = __fmaf_rn(-diff, rcp_approx(dist), a1);
-                }
+                if (has0) k9_guarded_term(diff, delta, k0, eps, a0);
+                if (has1) k9_guarded_term(diff, delta, k1, eps, a1);
             }
-            const int edge_l = pass >> 1;
-            const int gl0 = edge_l * 2 + (1 - axis), gl1 = ((edge_l == 2) ? 0 : edge_l + 1) * 2 + (1 - axis);
-#pragma unroll
-            for (int k = 0; k < 6; k++) {
-                if (k == gl0) gacc[k] += a0;
-                if (k == gl1) gacc[k] += a1;
-            }
+            k9_add_slots(pass, a0, a1, gacc);
             in_from = 1; in_to = 0;   // done
         }
         const unsigned todo = __ballot_sync(FULL, out_from <= out_to || in_from <= in_to);
@@ -664,13 +642,7 @@ k_nmr_backward_pixel_map(const float* __restrict__ faces, const int* __restrict_
         float acc0 = 0.f, acc1 = 0.f;   // contributions to vertex pi0 / pi1 of the current pass's edge, coordinate (1 - axis)
         auto flush = [&]() {
             if (cur_pass < 0) return;
-            const int e_ = cur_pass >> 1, ax_ = cur_pass & 1;
-            const int g0 = e_ * 2 + (1 - ax_), g1 = ((e_ == 2) ? 0 : e_ + 1) * 2 + (1 - ax_);
-#pragma unroll
-            for (int k = 0; k < 6; k++) {
-                if (k == g0) gacc[k] += acc0;
-                if (k == g1) gacc[k] += acc1;
-            }
+            k9_add_slots(cur_pass, acc0, acc1, gacc);
             acc0 = 0.f; acc1 = 0.f;
         };
         for (unsigned m = todo; m != 0u; m &= m - 1u) {
@@ -690,14 +662,14 @@ k_nmr_backward_pixel_map(const float* __restrict__ faces, const int* __restrict_
                 const float r0 = __shfl_sync(FULL, i0, src), r1 = __shfl_sync(FULL, i1, src), r2 = __shfl_sync(FULL, i2, src);
                 const float ra = (MODE & 2) ? __shfl_sync(FULL, ia, src) : 0.f;
                 if (both) k9_scan_out<MODE>(prow, s_of, s_ot, lane, r0, r1, r2, ra, s_cross, s_k0, s_k1, eps, acc0, acc1);
-                else k9_scan<MODE, false, false>(prow, nullptr, 0, s_of, s_ot, lane, fn, r0, r1, r2, ra, s_cross, s_k0, s_k1, (s_flags & 1) != 0, (s_flags & 2) != 0, eps, acc0, acc1);
+                else k9_scan<MODE, false>(prow, nullptr, 0, s_of, s_ot, lane, fn, r0, r1, r2, ra, s_cross, s_k0, s_k1, (s_flags & 1) != 0, (s_flags & 2) != 0, eps, acc0, acc1);
             }
             if (s_if <= s_it) {   // inwards up to the opposite edge, pixels owned by the face; reference colour = the out-pixel's
                 const float r0 = __shfl_sync(FULL, o0, src), r1 = __shfl_sync(FULL, o1, src), r2 = __shfl_sync(FULL, o2, src);
                 const float ra = (MODE & 2) ? __shfl_sync(FULL, oa, src) : 0.f;
                 const int s_stride = (s_axis == 0) ? is : 1;
                 const int* __restrict__ frow = fim_img + ((s_axis == 0) ? s_d0 : s_d0 * is);
-                k9_scan<MODE, true, false>(prow, frow, s_stride, s_if, s_it, lane, fn, r0, r1, r2, ra, s_cross, s_k0, s_k1, (s_flags & 1) != 0, (s_flags & 2) != 0, eps, acc0, acc1);
+                k9_scan<MODE, true>(prow, frow, s_stride, s_if, s_it, lane, fn, r0, r1, r2, ra, s_cross, s_k0, s_k1, (s_flags & 1) != 0, (s_flags & 2) != 0, eps, acc0, acc1);
             }
         }
         flush();

@@ -12,8 +12,8 @@ Forward: every map is bit-exact, as in tests/test_nmr_gpu.py.
 Gradients are held per face and per slot against oracle.nmr.backward_stats (u = 2^-24):
 
 K9.  The kernel's term for one visited pixel is d_k * rcp(dist_k), the reference's is fl(diff / dist).
-  * diff.  The kernel forms A = sum_k map_k g_k (k_nmr_pack, <= 4 FMAs) and then A - sum_k ref_k g_k (<= 4 FMAs; the
-    lane-serial inward loop: a product, <= 3 FMAs and a subtraction): <= 8 roundings, each below u * S with
+  * diff.  The kernel forms A = sum_k map_k g_k (k_nmr_pack, <= 4 FMAs) and then A - sum_k ref_k g_k (k9_diff,
+    <= 4 FMAs, in every scan): <= 8 roundings, each below u * S with
     S = sum_k |map_k g_k| + |ref_k g_k|.  The reference rounds (map - ref), the product and <= 3 partial sums: <= 5 u S.
     So |d_k - diff| <= 13 u S, also where one side is <= 0 and its term is skipped.  Summed over the visited pixels
     this is 13 u R, with R = sum S / |dist| (the scale 1 / |dist_k| differs from 1 / |dist| by O(u));
