@@ -43,6 +43,14 @@ def lib():
             C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
             C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_float, C.c_float,
             C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+        _lib.softras_oracle_backward_stats.restype = C.c_long
+        _lib.softras_oracle_backward_stats.argtypes = [
+            f32p, f32p, f32p, f32p, f32p, i32p, f32p,
+            C.POINTER(C.c_double), C.POINTER(C.c_double), i32p, C.POINTER(C.c_double),
+            C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+            C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_float, C.c_float,
+            C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+            f32p, C.POINTER(C.c_int64), C.c_long]
         _lib.softras_oracle_max_threads.restype = C.c_int
     return _lib
 
@@ -98,9 +106,17 @@ def forward(face_vertices, textures, params, rows=None, nthreads=0, row_stride=1
 
 
 def backward(face_vertices, textures, fwd, grad_soft_colors, params, accumulate_double=True, rows=None, row_stride=1,
-             nthreads=1):
+             nthreads=1, stats=False, exact_tail=False, nudge=0, terms=False):
     """Top-K backward (K6).  `fwd` is the dict returned by forward().  -> (grad_faces, grad_textures).
-    nthreads > 1 (CPU-baseline timing only): rows are dealt to threads with private double accumulators."""
+    nthreads > 1 (CPU-baseline timing only): rows are dealt to threads with private double accumulators.
+
+    stats=True: -> (faces, textures), each a dict of float64 / int32 arrays shaped like the gradient: g64 (the double
+    sum of the reference's float terms, which accumulate_double rounds), A (sum of |term|), N (number of non-zero terms)
+    and E (sum over terms of how far the CUDA kernel's term may be from the reference's, see softras_oracle.c's
+    rounding sites; exact_tail is the kernel's softras_exact_tail option).  N counts the pairs that write a term into the
+    entry, zero or not: at least as many as the float additions the kernel makes into it.  terms=True adds 'terms': (values, slots)
+    of every non-zero term in the sequential order, slots indexing the faces then the textures gradient, flattened.
+    nudge = +1 / -1 / 2 computes g64 with every rounding site moved by its budget up / down / by a hashed sign."""
     fv = np.ascontiguousarray(face_vertices, dtype=np.float32)
     tx = np.ascontiguousarray(textures, dtype=np.float32)
     g = np.ascontiguousarray(grad_soft_colors, dtype=np.float32)
@@ -111,6 +127,8 @@ def backward(face_vertices, textures, fwd, grad_soft_colors, params, accumulate_
     gf = np.zeros((B, nf, 3, 3), np.float32)
     gt = np.zeros((B, nf, T, 3), np.float32)
     r0, r1 = (0, H) if rows is None else rows
+    if stats:
+        return _backward_stats(fv, tx, fwd, g, params, (r0, r1), int(row_stride), exact_tail, nudge, terms)
     if nthreads > 1:
         lib().softras_oracle_backward_mt(
             _p(fv, C.c_float), _p(tx, C.c_float), _p(np.ascontiguousarray(fwd["soft_colors"]), C.c_float),
@@ -125,6 +143,60 @@ def backward(face_vertices, textures, fwd, grad_soft_colors, params, accumulate_
         _p(gf, C.c_float), _p(gt, C.c_float), B, nf, T, H, K, *params.scalars(),
         int(bool(accumulate_double)), r0, r1, int(row_stride))
     return gf, gt
+
+
+def _backward_stats(fv, tx, fwd, g, params, rows, row_stride, exact_tail, nudge, terms):
+    B, nf = fv.shape[:2]
+    T = tx.shape[2]
+    H = int(params["image_size"])
+    K = int(params["max_faces_per_pixel_for_grad"])
+    ngf, ngt = B * nf * 9, B * nf * T * 3
+    g64, A, E = (np.zeros(ngf + ngt) for _ in range(3))
+    N = np.zeros(ngf + ngt, np.int32)
+    ins = [_p(fv, C.c_float), _p(tx, C.c_float), _p(np.ascontiguousarray(fwd["soft_colors"]), C.c_float),
+           _p(np.ascontiguousarray(fwd["faces_info"]), C.c_float), _p(np.ascontiguousarray(fwd["aggrs_info"]), C.c_float),
+           _p(np.ascontiguousarray(fwd["faces_id_buffer"]), C.c_int32), _p(g, C.c_float)]
+    outs = [_p(g64, C.c_double), _p(A, C.c_double), _p(N, C.c_int32), _p(E, C.c_double)]
+    args = [B, nf, T, H, K, *params.scalars(), int(bool(exact_tail)), int(nudge), rows[0], rows[1], row_stride]
+    n = lib().softras_oracle_backward_stats(*ins, *outs, *args, None, None, 0)
+    res = [dict(g64=x[:ngf].reshape(B, nf, 3, 3), A=a[:ngf].reshape(B, nf, 3, 3), N=c[:ngf].reshape(B, nf, 3, 3),
+                E=e[:ngf].reshape(B, nf, 3, 3)) for x, a, c, e in [(g64, A, N, E)]]
+    res.append(dict(g64=g64[ngf:].reshape(B, nf, T, 3), A=A[ngf:].reshape(B, nf, T, 3), N=N[ngf:].reshape(B, nf, T, 3),
+                    E=E[ngf:].reshape(B, nf, T, 3)))
+    if terms:
+        val, slot = np.zeros(n, np.float32), np.zeros(n, np.int64)
+        lib().softras_oracle_backward_stats(*ins, *outs, *args, _p(val, C.c_float), _p(slot, C.c_int64), n)
+        res[0]["terms"] = (val, slot)
+    return tuple(res)
+
+
+U = 2.0 ** -24      # fp32 unit roundoff
+FTZ = 2.0 ** -125   # twice the smallest normal fp32
+
+
+def backward_bound(st):
+    """Per-entry bound on |CUDA gradient - g64| for one stats dict of backward(stats=True):
+
+        bound = E * (1 + gamma) + gamma * A + N * 2^-125,   gamma = N u / (1 - N u),  u = 2^-24.
+
+    Derivation.  The kernel's terms t'_i of a slot differ from the reference's float terms t_i by at most the
+    per-site budgets, so sum |t'_i - t_i| <= E and sum |t'_i| <= A + E.  The kernel adds the t'_i in float, in some
+    binary tree whatever the grouping: the shuffle merges between lanes, the vector and scalar atomics, any
+    regrouping.  Starting from the zeroed accumulator, a tree of at most N float additions (adding a zero is exact) is
+    within gamma_{N-1} sum |t'_i| of their exact sum (Higham, Accuracy and Stability
+    of Numerical Algorithms, 4.2), independent
+    of the order.  g64 is the same sum over the t_i in double, within N 2^-53 A of exact; gamma_N - gamma_{N-1} >= u
+    covers that and the E gamma term is second order.  So
+        |got - g64| <= E + gamma_{N-1} (A + E) + N 2^-53 A <= E (1 + gamma_N) + gamma_N A,
+    which in the form 2^-24 (N + c) A has c = N^2 u / (1 - N u), below 1 for N < 4096.  The finalize kernel copies
+    the accumulator into grad_faces / grad_textures unchanged, so no rounding follows the sum.  The global float
+    atomics flush subnormal inputs and results to zero (PTX red.add.f32): each of at most N atomic adds into the slot
+    loses < 2^-126 on its input and < 2^-126 on its result, hence the N 2^-125 floor, which only matters for sums in
+    the subnormal range.  Non-finite entries are not bounded: compare their NaN / inf pattern instead."""
+    N = st["N"].astype(np.float64)
+    gamma = N * U / (1.0 - N * U)
+    with np.errstate(invalid="ignore"):
+        return st["E"] * (1.0 + gamma) + gamma * st["A"] + N * FTZ
 
 
 def max_threads():

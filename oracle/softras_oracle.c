@@ -53,6 +53,66 @@
 
 #define K_MAX_POINTS_PER_PIXEL 64 /* :16 */
 
+/* ------------------------------------------------------------------ rounding sites of the K6 backward
+ * The CUDA backward computes every (pixel, face) term with this file's arithmetic except at the sites below, where it
+ * may round differently.  softras_oracle_backward_stats re-evaluates each pair with its live sites moved by their
+ * budgets in units in the last place (jointly, see there) to bound how far the kernel's term can be from this one:
+ *   SITE_EXP_SIG   expf in the sigmoid: libm and CUDA's expf are each within 2 ulp of exp, so <= 3 ulp apart
+ *                  (2 + 1 for a libm that is only faithful).
+ *   SITE_EXP_SOFT  expf in the softmax weight, likewise.
+ *   SITE_TAIL_D    softras_exact_tail = 0: D = 1 / (1 + e) in two fp32 roundings (each <= 2^-24 relative, < 1 ulp
+ *                  together) against one rounding of the double quotient (<= 1/2 ulp): <= 2 ulp.
+ *   SITE_PROD      softras_exact_tail = 0: the alpha-prod factor g * ((1 - alpha) / max(1 - D, 1e-6f)) in two fp32
+ *                  roundings (< 2 ulp), a numerator below 2^-60 (one more ulp, as the divisions below), the double
+ *                  1e-6 against 1e-6f (2.5e-9 relative) and the reference's one rounding (1/2 ulp): <= 4 ulp.
+ *   SITE_DIV + i   softras_exact_tail = 0: the kernel's relaxed divisions are bit-exact for numerators >= 2^-60
+ *                  (exact_math.cuh) and within 1 ulp below; a site is live only for a non-zero numerator < 2^-60.
+ * With softras_exact_tail = 1 the tails and divisions are the reference's bit for bit and only the two expf sites
+ * remain. */
+enum {
+    SITE_EXP_SIG, SITE_EXP_SOFT, SITE_TAIL_D, SITE_PROD,
+    SITE_DIV_SIGARG, SITE_DIV_ZSOFT, SITE_DIV_COLD, SITE_DIV_GAMMA, SITE_DIV_NMF, SITE_DIV_SIGMA,
+    SITE_DIV_Z1,          /* + k, k < 3: (C * w_k) / z_k */
+    SITE_DIV_Z2 = SITE_DIV_Z1 + 3,      /* + k: (.. / z_k) / z_k */
+    SITE_DIV_CLIPW = SITE_DIV_Z2 + 3,   /* + k: w_k / w_sum */
+    SITE_DIV_CLIPZ = SITE_DIV_CLIPW + 3, /* + k: w_k / z_k inside zp */
+    SITE_DIV_EUC = SITE_DIV_CLIPZ + 3,  /* + k: the euclidean edge parameter of edge k */
+    N_SITES = SITE_DIV_EUC + 3
+};
+typedef struct {
+    int exact_tail;       /* the kernel's softras_exact_tail */
+    uint32_t up, down;    /* sites moved up / down by their budget */
+    int hashed;           /* every live site moved, by a hashed sign per (pair, site) */
+    uint32_t pair;        /* hash input */
+    uint32_t live;        /* out: sites with a non-zero budget in this pair */
+} Nudge;
+
+static inline float move_ulps(float x, int n, int dir) {
+    for (int i = 0; i < n; i++) x = nextafterf(x, dir > 0 ? INFINITY : -INFINITY);
+    return x;
+}
+
+/* x at site s with a budget of n ulp */
+static inline float site(Nudge *nd, int s, float x, int n) {
+    if (!nd || n <= 0 || !isfinite(x)) return x;
+    nd->live |= 1u << s;
+    if (nd->up >> s & 1u) return move_ulps(x, n, 1);
+    if (nd->down >> s & 1u) return move_ulps(x, n, -1);
+    if (nd->hashed) {
+        uint32_t h = nd->pair * 0x9E3779B1u ^ (uint32_t)(s + 1) * 0x85EBCA77u;
+        h ^= h >> 15; h *= 0x2C1B3C6Du; h ^= h >> 12;
+        return move_ulps(x, n, (h & 1u) ? 1 : -1);
+    }
+    return x;
+}
+
+/* a / b as one of the kernel's relaxed divisions */
+static inline float rdiv(Nudge *nd, int s, float a, float b) {
+    const float q = a / b;
+    if (nd && !nd->exact_tail && a != 0.f && fabsf(a) < 0x1p-60f) return site(nd, s, q, 1);
+    return q;
+}
+
 /* :20-25 */
 static inline void barycentric_coordinate(float *w, float x, float y, const float *fi) {
     w[0] = fi[0] * x + fi[1] * y + fi[2];
@@ -85,11 +145,11 @@ static inline void barycentric_clip(float *w) {
     for (int k = 0; k < 3; k++) w[k] /= w_sum;
 }
 
-/* :57-147 */
+/* :57-147.  nd: the backward's rounding sites (NULL in the forward, whose divisions are exact) */
 static inline void euclidean_p2f_distance(float *sign, float *dis_x, float *dis_y,
                                           const float *w, float *t,
                                           const float *face, const float *face_info,
-                                          float xp, float yp) {
+                                          float xp, float yp, Nudge *nd) {
     const float *face_sym = face_info + 9;
     const float *face_obt = face_info + 18;
 
@@ -107,7 +167,7 @@ static inline void euclidean_p2f_distance(float *sign, float *dis_x, float *dis_
             a0[1] = face_sym[3 * v0 + 1] - face_sym[3 * v1 + 1];
             a0[2] = face_sym[3 * v0 + 2] - face_sym[3 * v1 + 2];
 
-            t0[v0] = (w[0] * a0[0] + w[1] * a0[1] + w[2] * a0[2] - a0[v1]) / (a0[v0] - a0[v1]);
+            t0[v0] = rdiv(nd, SITE_DIV_EUC + k, w[0] * a0[0] + w[1] * a0[1] + w[2] * a0[2] - a0[v1], a0[v0] - a0[v1]);
             t0[v1] = 1 - t0[v0];
             t0[v2] = 0;
 
@@ -157,7 +217,7 @@ static inline void euclidean_p2f_distance(float *sign, float *dis_x, float *dis_
         a0[1] = face_sym[3 * v0 + 1] - face_sym[3 * v1 + 1];
         a0[2] = face_sym[3 * v0 + 2] - face_sym[3 * v1 + 2];
 
-        t[v0] = (w[0] * a0[0] + w[1] * a0[1] + w[2] * a0[2] - a0[v1]) / (a0[v0] - a0[v1]);
+        t[v0] = rdiv(nd, SITE_DIV_EUC + v0, w[0] * a0[0] + w[1] * a0[1] + w[2] * a0[2] - a0[v1], a0[v0] - a0[v1]);
         t[v1] = 1 - t[v0];
         t[v2] = 0;
 
@@ -374,7 +434,7 @@ static void forward_rows(const float *faces, const float *textures, const float 
                     if (-dis >= threshold) continue;
                     soft_fragment = (float)(1. / (1. + (double)expf(-dis / sigma_val)));
                 } else {
-                    euclidean_p2f_distance(&sign, &dis_x, &dis_y, w, t, face, face_info, xp, yp);
+                    euclidean_p2f_distance(&sign, &dis_x, &dis_y, w, t, face, face_info, xp, yp, NULL);
                     dis = dis_x * dis_x + dis_y * dis_y;
                     if (sign < 0 && dis >= threshold) continue;
                     soft_fragment = (float)(1. / (1. + (double)expf(-sign * dis / sigma_val)));
@@ -483,7 +543,173 @@ void softras_oracle_forward(const float *faces, const float *textures, float *fa
 }
 
 /* ------------------------------------------------------------------ K6 :1177-1360
- * Sequential restatement: pixels in ascending linear index, slots m ascending,
+ * The terms of one (pixel, face) pair: gv[k*3+l] for grad_faces[fn][k][l]; when it returns 1, gtex[3*j+k] for
+ * grad_textures[fn][j][k] (j < texture_size; 0 for texels the pair does not hit).  nd: rounding sites (NULL: none). */
+typedef struct {
+    int nf, texture_size, texture_res, func_id_dist, func_id_rgb, func_id_alpha, texture_sample_type;
+    float near, far, sigma_val, gamma_val;
+} BwdParams;
+
+static int pair_terms(const BwdParams *P, const float *face, const float *texture, const float *face_info, int fn,
+                      float xp, float yp, const float g[4], const float oc[4], float softmax_sum, float softmax_max,
+                      Nudge *nd, float gv[9], float *gtex) {
+    const int texture_size = P->texture_size, texture_res = P->texture_res, texture_sample_type = P->texture_sample_type;
+    const float near = P->near, far = P->far, sigma_val = P->sigma_val, gamma_val = P->gamma_val;
+    float dis = 0, dis_x = 0, dis_y = 0, t[3] = {0, 0, 0}, w[3], w0[3], sign = 0, soft_fragment;
+    int tex_written = 0;
+
+    barycentric_coordinate(w, xp, yp, face_info);
+
+    if (P->func_id_dist == 0) {
+        soft_fragment = 1;
+    } else {
+        float x;
+        if (P->func_id_dist == 1) {
+            dis = forward_barycentric_p2f_distance(w);
+            for (int k = 0; k < 3; k++) t[k] = w[k];
+            x = rdiv(nd, SITE_DIV_SIGARG, -dis, sigma_val);
+        } else {
+            euclidean_p2f_distance(&sign, &dis_x, &dis_y, w, t, face, face_info, xp, yp, nd);
+            dis = dis_x * dis_x + dis_y * dis_y;
+            x = rdiv(nd, SITE_DIV_SIGARG, -sign * dis, sigma_val);
+        }
+        const float e = fmaxf(site(nd, SITE_EXP_SIG, expf(x), 3), 0.f);
+        soft_fragment = (float)(1. / (1. + (double)e));
+        if (nd && !nd->exact_tail) soft_fragment = fminf(fmaxf(site(nd, SITE_TAIL_D, soft_fragment, 2), 0.f), 1.f);
+    }
+
+    float grad_v[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
+    float C_grad_xy = 0;
+
+    float C_grad_xy_alpha = g[3];
+    if (P->func_id_alpha == 0) {
+    } else if (P->func_id_alpha == 1) {
+        C_grad_xy_alpha /= P->nf;
+    } else if (P->func_id_alpha == 2) {
+        C_grad_xy_alpha = (float)((double)C_grad_xy_alpha * ((double)(1 - oc[3]) / fmax((double)(1 - soft_fragment), 1e-6)));
+        if (nd && !nd->exact_tail) C_grad_xy_alpha = site(nd, SITE_PROD, C_grad_xy_alpha, 4);
+    }
+    C_grad_xy += C_grad_xy_alpha;
+
+    for (int k = 0; k < 3; k++) w0[k] = w[k];
+    /* barycentric_clip (:49-54) and zp (:1296) */
+    for (int k = 0; k < 3; k++) w[k] = (float)fmax(fmin((double)w[k], 1.), 0.);
+    const float w_sum = (float)fmax((double)(w[0] + w[1] + w[2]), 1e-5);
+    for (int k = 0; k < 3; k++) w[k] = rdiv(nd, SITE_DIV_CLIPW + k, w[k], w_sum);
+    const float zp = (float)(1. / (double)(rdiv(nd, SITE_DIV_CLIPZ + 0, w[0], face[2]) + rdiv(nd, SITE_DIV_CLIPZ + 1, w[1], face[5]) +
+                                           rdiv(nd, SITE_DIV_CLIPZ + 2, w[2], face[8])));
+
+    if (P->func_id_rgb == 0) {
+        if ((float)fn == softmax_max) { /* int vs float compare, Q10 */
+            tex_written = 1;
+            for (int k = 0; k < 3; k++)
+                for (int j = 0; j < texture_size; j++)
+                    gtex[3 * j + k] = backward_sample_texture(g[k], w, texture_res, j, texture_sample_type);
+        }
+    } else if (P->func_id_rgb == 1) {
+        tex_written = 1;
+        float C_grad_xyz_rgb = 0.f;
+        const float zp_norm = (far - zp) / (far - near);
+        const float e = fmaxf(site(nd, SITE_EXP_SOFT, expf((zp_norm - softmax_max) / gamma_val), 3), 0.f);
+        const float zp_softmax = rdiv(nd, SITE_DIV_ZSOFT, soft_fragment * e, softmax_sum);
+
+        for (int k = 0; k < 3; k++) {
+            for (int j = 0; j < texture_size; j++)
+                gtex[3 * j + k] = zp_softmax * backward_sample_texture(g[k], w, texture_res, j, texture_sample_type);
+            const float color_k = forward_sample_texture_bwd(texture, w, texture_res, k, texture_sample_type);
+            C_grad_xyz_rgb += g[k] * (color_k - oc[k]);
+        }
+        C_grad_xyz_rgb *= zp_softmax;
+        C_grad_xy += rdiv(nd, SITE_DIV_COLD, C_grad_xyz_rgb, soft_fragment);
+
+        const float C_grad_z_rgb = rdiv(nd, SITE_DIV_NMF, rdiv(nd, SITE_DIV_GAMMA, C_grad_xyz_rgb, gamma_val), near - far) * zp * zp;
+        for (int k = 0; k < 3; k++)
+            grad_v[k][2] = rdiv(nd, SITE_DIV_Z2 + k, rdiv(nd, SITE_DIV_Z1 + k, C_grad_z_rgb * w[k], face[3 * k + 2]), face[3 * k + 2]);
+    }
+
+    C_grad_xy *= rdiv(nd, SITE_DIV_SIGMA, soft_fragment * (1 - soft_fragment), sigma_val);
+    if (P->func_id_dist == 1) {
+        backward_barycentric_p2f_distance(grad_v, t, face_info, xp, yp, dis, C_grad_xy);
+    } else if (P->func_id_dist == 2) {
+        for (int k = 0; k < 3; k++)
+            for (int l = 0; l < 2; l++)
+                grad_v[k][l] = 2 * sign * C_grad_xy * (t[k] + w0[k]) * (l == 0 ? dis_x : dis_y);
+    }
+    for (int k = 0; k < 3; k++)
+        for (int l = 0; l < 3; l++) gv[3 * k + l] = grad_v[k][l];
+    return tex_written;
+}
+
+/* Walks the pairs of K6 in the reference's sequential order (pixels in ascending linear index, slots m ascending)
+ * and hands each one's terms to visit(). */
+typedef void (*PairVisitor)(void *ctx, const BwdParams *P, const float *face, const float *texture,
+                            const float *face_info, int fn, long pair, float xp, float yp, const float g[4],
+                            const float oc[4], float softmax_sum, float softmax_max, size_t gfo, size_t gto);
+
+static void walk_pairs(const float *faces, const float *textures, const float *soft_colors, const float *faces_info,
+                       const float *aggrs_info, const int32_t *faces_id_buffer, const float *grad_soft_colors,
+                       const BwdParams *P, int batch_size, int image_size, int max_faces_id, float threshold,
+                       int row_begin, int row_end, int row_stride, PairVisitor visit, void *ctx) {
+    const int is = image_size, nf = P->nf, mf = max_faces_id, texture_size = P->texture_size;
+    const long npix = (long)is * is;
+    for (int bn = 0; bn < batch_size; bn++)
+        for (int row = row_begin; row < row_end; row += (row_stride < 1 ? 1 : row_stride))
+            for (int col = 0; col < is; col++) {
+                const long pn = (long)row * is + col;
+                const int yi = is - 1 - row;
+                const int xi = col;
+                const float yp = (float)((2. * yi + 1 - is) / is);
+                const float xp = (float)((2. * xi + 1 - is) / is);
+                const float softmax_sum = aggrs_info[((long)bn * 2 + 0) * npix + pn];
+                const float softmax_max = aggrs_info[((long)bn * 2 + 1) * npix + pn];
+                float g[4], oc[4];
+                for (int k = 0; k < 4; k++) {
+                    g[k] = grad_soft_colors[((long)bn * 4 + k) * npix + pn];
+                    oc[k] = soft_colors[((long)bn * 4 + k) * npix + pn];
+                }
+                for (int m = 0; m < mf; m++) {
+                    const int fn = faces_id_buffer[((long)bn * mf + m) * npix + pn];
+                    if (fn == -1) break;
+                    const float *face = &faces[((long)bn * nf + fn) * 9];
+                    if (check_border(xp, yp, face, sqrtf(threshold))) continue;
+                    visit(ctx, P, face, &textures[((long)bn * nf + fn) * texture_size * 3],
+                          &faces_info[((long)bn * nf + fn) * 27], fn, ((long)bn * npix + pn) * mf + m, xp, yp, g, oc,
+                          softmax_sum, softmax_max, ((size_t)bn * nf + fn) * 9, ((size_t)bn * nf + fn) * texture_size * 3);
+                }
+            }
+}
+
+static BwdParams bwd_params(int num_faces, int texture_size, float near, float far, float sigma_val, int func_id_dist,
+                            float gamma_val, int func_id_rgb, int func_id_alpha, int texture_sample_type) {
+    BwdParams P = {num_faces, texture_size, (int)sqrt((double)texture_size), func_id_dist, func_id_rgb, func_id_alpha,
+                   texture_sample_type, near, far, sigma_val, gamma_val};
+    return P;
+}
+
+typedef struct {
+    int accumulate_double;
+    double *gf, *gt;
+    float *gtex;
+} SumCtx;
+
+static void acc(const SumCtx *c, double *buf, size_t idx, float val) {
+    if (c->accumulate_double) buf[idx] += (double)val;
+    else buf[idx] = (double)((float)buf[idx] + val);
+}
+
+static void sum_pair(void *ctx, const BwdParams *P, const float *face, const float *texture, const float *face_info,
+                     int fn, long pair, float xp, float yp, const float g[4], const float oc[4], float softmax_sum,
+                     float softmax_max, size_t gfo, size_t gto) {
+    SumCtx *c = (SumCtx *)ctx;
+    float gv[9];
+    (void)pair;
+    const int tw = pair_terms(P, face, texture, face_info, fn, xp, yp, g, oc, softmax_sum, softmax_max, NULL, gv, c->gtex);
+    if (tw)
+        for (int j = 0; j < 3 * P->texture_size; j++) acc(c, c->gt, gto + j, c->gtex[j]);
+    for (int i = 0; i < 9; i++) acc(c, c->gf, gfo + i, gv[i]);
+}
+
+/* Sequential restatement: pixels in ascending linear index, slots m ascending,
  * `+=` in place of atomicAdd.  accumulate_double != 0 accumulates in double and
  * rounds once at the end (order-free centre for tolerance tests); 0 accumulates
  * in float exactly like a serialised execution of the reference.
@@ -500,135 +726,139 @@ void softras_oracle_backward(const float *faces, const float *textures, const fl
                              int row_begin, int row_end, int row_stride) {
     (void)eps;
     (void)double_side;
-    const int is = image_size;
-    const int nf = num_faces;
-    const int mf = max_faces_id;
-    const long npix = (long)is * is;
-    const int texture_res = (int)sqrt((double)texture_size);
-    const float threshold = dist_eps * sigma_val;
-    const size_t ngf = (size_t)batch_size * nf * 9;
-    const size_t ngt = (size_t)batch_size * nf * texture_size * 3;
-    double *gf = (double *)calloc(ngf, sizeof(double));
-    double *gt = (double *)calloc(ngt, sizeof(double));
-#define ACC(buf, idx, val)                                                   \
-    do {                                                                     \
-        if (accumulate_double) buf[idx] += (double)(val);                    \
-        else buf[idx] = (double)((float)buf[idx] + (float)(val));            \
-    } while (0)
+    const BwdParams P = bwd_params(num_faces, texture_size, near, far, sigma_val, func_id_dist, gamma_val, func_id_rgb,
+                                   func_id_alpha, texture_sample_type);
+    const size_t ngf = (size_t)batch_size * num_faces * 9;
+    const size_t ngt = (size_t)batch_size * num_faces * texture_size * 3;
+    SumCtx c = {accumulate_double, (double *)calloc(ngf, sizeof(double)), (double *)calloc(ngt, sizeof(double)),
+                (float *)malloc(sizeof(float) * 3 * (size_t)texture_size)};
+    walk_pairs(faces, textures, soft_colors, faces_info, aggrs_info, faces_id_buffer, grad_soft_colors, &P, batch_size,
+               image_size, max_faces_id, dist_eps * sigma_val, row_begin, row_end, row_stride, sum_pair, &c);
+    for (size_t i = 0; i < ngf; i++) grad_faces[i] = (float)c.gf[i];
+    for (size_t i = 0; i < ngt; i++) grad_textures[i] = (float)c.gt[i];
+    free(c.gf);
+    free(c.gt);
+    free(c.gtex);
+}
 
-    for (int bn = 0; bn < batch_size; bn++)
-        for (int row = row_begin; row < row_end; row += (row_stride < 1 ? 1 : row_stride))
-            for (int col = 0; col < is; col++) {
-                const long pn = (long)row * is + col;
-                const int yi = is - 1 - row;
-                const int xi = col;
-                const float yp = (float)((2. * yi + 1 - is) / is);
-                const float xp = (float)((2. * xi + 1 - is) / is);
+/* Per-slot statistics of the K6 terms, over slots s = grad_faces index (< B*nf*9), then B*nf*9 + grad_textures index:
+ *   g64[s]  double sum of the terms (what accumulate_double = 1 rounds),
+ *   A[s]    sum of |term|,
+ *   N[s]    number of pairs that write a term into the slot, zero or not: at least as many as the float additions the
+ *           kernel makes into it,
+ *   E[s]    sum over pairs of how far the kernel's term may be from this one: the largest |term moved - term| over
+ *           the moves of the pair's first six live rounding sites to the corners of their budget box and of each site
+ *           alone, plus, for every further live site (tiny-numerator divisions only), its own largest move.
+ *           A term is monotone in each site's value within its budget except across a clamp, so its extremes over
+ *           the box lie on those points.  Sites interact (moving expf can make a division site live, and D's and
+ *           1 - D's roundings compound near D = 1), so the corners are taken jointly, not site by site.
+ * exact_tail: the kernel's softras_exact_tail.  nudge: 0, or +1 / -1 / 2 to compute g64 (only) with every live site
+ * moved by its budget up / down / by a hashed sign per pair and site.  term_val / term_slot (NULL or term_cap
+ * entries): every non-zero term and its slot, in the sequential order. */
+#define MAX_CORNER_SITES 6
+typedef struct {
+    int exact_tail, nudge;
+    size_t ngf;
+    double *g64, *A, *E;
+    int32_t *N;
+    float *base, *moved, *dmax, *dextra;
+    float *term_val;
+    int64_t *term_slot;
+    long term_cap, nterms;
+} StatsCtx;
 
-                const float softmax_sum = aggrs_info[((long)bn * 2 + 0) * npix + pn];
-                const float softmax_max = aggrs_info[((long)bn * 2 + 1) * npix + pn];
-
-                for (int m = 0; m < mf; m++) {
-                    const int fn = faces_id_buffer[((long)bn * mf + m) * npix + pn];
-                    if (fn == -1) break;
-
-                    const float *face = &faces[((long)bn * nf + fn) * 9];
-                    const float *texture = &textures[((long)bn * nf + fn) * texture_size * 3];
-                    const float *face_info = &faces_info[((long)bn * nf + fn) * 27];
-
-                    if (check_border(xp, yp, face, sqrtf(threshold))) continue;
-
-                    float dis = 0, dis_x = 0, dis_y = 0, t[3] = {0, 0, 0}, w[3], w0[3], sign = 0, soft_fragment;
-
-                    barycentric_coordinate(w, xp, yp, face_info);
-
-                    if (func_id_dist == 0) {
-                        soft_fragment = 1;
-                    } else if (func_id_dist == 1) {
-                        dis = forward_barycentric_p2f_distance(w);
-                        for (int k = 0; k < 3; k++) t[k] = w[k];
-                        soft_fragment = (float)(1. / (1. + (double)expf(-dis / sigma_val)));
-                    } else {
-                        euclidean_p2f_distance(&sign, &dis_x, &dis_y, w, t, face, face_info, xp, yp);
-                        dis = dis_x * dis_x + dis_y * dis_y;
-                        soft_fragment = (float)(1. / (1. + (double)expf(-sign * dis / sigma_val)));
-                    }
-
-                    const size_t gfo = ((size_t)bn * nf + fn) * 9;
-                    const size_t gto = ((size_t)bn * nf + fn) * texture_size * 3;
-                    float grad_v[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
-                    float C_grad_xy = 0;
-
-                    float C_grad_xy_alpha = grad_soft_colors[((long)bn * 4 + 3) * npix + pn];
-                    if (func_id_alpha == 0) {
-                    } else if (func_id_alpha == 1) {
-                        C_grad_xy_alpha /= nf;
-                    } else if (func_id_alpha == 2) {
-                        C_grad_xy_alpha = (float)((double)C_grad_xy_alpha *
-                                                  ((double)(1 - soft_colors[((long)bn * 4 + 3) * npix + pn]) /
-                                                   fmax((double)(1 - soft_fragment), 1e-6)));
-                    }
-                    C_grad_xy += C_grad_xy_alpha;
-
-                    for (int k = 0; k < 3; k++) w0[k] = w[k];
-                    barycentric_clip(w);
-                    const float zp = (float)(1. / (double)(w[0] / face[2] + w[1] / face[5] + w[2] / face[8]));
-
-                    if (func_id_rgb == 0) {
-                        if ((float)fn == softmax_max) { /* int vs float compare, Q10 */
-                            for (int k = 0; k < 3; k++)
-                                for (int j = 0; j < texture_size; j++)
-                                    ACC(gt, gto + 3 * j + k,
-                                        backward_sample_texture(grad_soft_colors[((long)bn * 4 + k) * npix + pn], w, texture_res, j, texture_sample_type));
-                        }
-                    } else if (func_id_rgb == 1) {
-                        float C_grad_xyz_rgb = 0.f;
-                        const float zp_norm = (far - zp) / (far - near);
-                        const float zp_softmax = soft_fragment * expf((zp_norm - softmax_max) / gamma_val) / softmax_sum;
-
-                        for (int k = 0; k < 3; k++) {
-                            const float grad_soft_color_k = grad_soft_colors[((long)bn * 4 + k) * npix + pn];
-                            for (int j = 0; j < texture_size; j++) {
-                                const float grad_t = backward_sample_texture(grad_soft_color_k, w, texture_res, j, texture_sample_type);
-                                ACC(gt, gto + 3 * j + k, zp_softmax * grad_t);
-                            }
-                            const float color_k = forward_sample_texture_bwd(texture, w, texture_res, k, texture_sample_type);
-                            C_grad_xyz_rgb += grad_soft_color_k * (color_k - soft_colors[((long)bn * 4 + k) * npix + pn]);
-                        }
-                        C_grad_xyz_rgb *= zp_softmax;
-                        C_grad_xy += C_grad_xyz_rgb / soft_fragment;
-
-                        const float C_grad_z_rgb = C_grad_xyz_rgb / gamma_val / (near - far) * zp * zp;
-                        grad_v[0][2] = C_grad_z_rgb * w[0] / face[2] / face[2];
-                        grad_v[1][2] = C_grad_z_rgb * w[1] / face[5] / face[5];
-                        grad_v[2][2] = C_grad_z_rgb * w[2] / face[8] / face[8];
-                    }
-
-                    C_grad_xy *= soft_fragment * (1 - soft_fragment) / sigma_val;
-                    if (func_id_dist == 1) {
-                        backward_barycentric_p2f_distance(grad_v, t, face_info, xp, yp, dis, C_grad_xy);
-                    } else if (func_id_dist == 2) {
-                        for (int k = 0; k < 3; k++)
-                            for (int l = 0; l < 2; l++)
-                                grad_v[k][l] = 2 * sign * C_grad_xy * (t[k] + w0[k]) * (l == 0 ? dis_x : dis_y);
-                    }
-
-                    ACC(gf, gfo + 0, grad_v[0][0]);
-                    ACC(gf, gfo + 1, grad_v[0][1]);
-                    ACC(gf, gfo + 3, grad_v[1][0]);
-                    ACC(gf, gfo + 4, grad_v[1][1]);
-                    ACC(gf, gfo + 6, grad_v[2][0]);
-                    ACC(gf, gfo + 7, grad_v[2][1]);
-                    ACC(gf, gfo + 2, grad_v[0][2]);
-                    ACC(gf, gfo + 5, grad_v[1][2]);
-                    ACC(gf, gfo + 8, grad_v[2][2]);
+static void stats_pair(void *ctx, const BwdParams *P, const float *face, const float *texture, const float *face_info,
+                       int fn, long pair, float xp, float yp, const float g[4], const float oc[4], float softmax_sum,
+                       float softmax_max, size_t gfo, size_t gto) {
+    StatsCtx *c = (StatsCtx *)ctx;
+    const int ns = 9 + 3 * P->texture_size;
+    Nudge nd = {c->exact_tail, 0, 0, c->nudge == 2, (uint32_t)pair, 0};
+    if (c->nudge == 1) nd.up = ~0u;
+    if (c->nudge == -1) nd.down = ~0u;
+    const int tw = pair_terms(P, face, texture, face_info, fn, xp, yp, g, oc, softmax_sum, softmax_max, &nd, c->base, c->base + 9);
+    const int nslots = tw ? ns : 9;
+    for (int i = 0; i < nslots; i++) c->dmax[i] = c->dextra[i] = 0.f;
+    if (!c->nudge && nd.live) {
+        int live[N_SITES], L = 0;
+        for (int s = 0; s < N_SITES; s++)
+            if (nd.live >> s & 1u) live[L++] = s;
+        const int Lc = L < MAX_CORNER_SITES ? L : MAX_CORNER_SITES;
+        const long ncorner = 1L << Lc;
+        for (long p = 0; p < ncorner + 2 * L; p++) {
+            Nudge n2 = {c->exact_tail, 0, 0, 0, (uint32_t)pair, 0};
+            if (p < ncorner) {
+                for (int i = 0; i < Lc; i++) {
+                    if (p >> i & 1L) n2.up |= 1u << live[i];
+                    else n2.down |= 1u << live[i];
                 }
+            } else if ((p - ncorner) & 1L) {
+                n2.up = 1u << live[(p - ncorner) >> 1];
+            } else {
+                n2.down = 1u << live[(p - ncorner) >> 1];
             }
-#undef ACC
-    for (size_t i = 0; i < ngf; i++) grad_faces[i] = (float)gf[i];
-    for (size_t i = 0; i < ngt; i++) grad_textures[i] = (float)gt[i];
-    free(gf);
-    free(gt);
+            pair_terms(P, face, texture, face_info, fn, xp, yp, g, oc, softmax_sum, softmax_max, &n2, c->moved, c->moved + 9);
+            float *d_out = c->dmax;
+            if (p >= ncorner && (int)((p - ncorner) >> 1) >= Lc) d_out = c->dextra;   /* a site past the corners */
+            for (int i = 0; i < nslots; i++) {
+                const float d = fabsf(c->moved[i] - c->base[i]);
+                if (!(d <= d_out[i])) d_out[i] = d;   /* NaN propagates */
+            }
+            if (d_out == c->dextra && ((p - ncorner) & 1L))   /* both directions of this site done */
+                for (int i = 0; i < nslots; i++) {
+                    c->E[i < 9 ? gfo + i : c->ngf + gto + (i - 9)] += c->dextra[i];
+                    c->dextra[i] = 0.f;
+                }
+        }
+    }
+    for (int i = 0; i < nslots; i++) {
+        const size_t s = i < 9 ? gfo + i : c->ngf + gto + (i - 9);
+        const float v = c->base[i];
+        c->g64[s] += (double)v;
+        c->E[s] += c->dmax[i];
+        c->N[s]++;
+        if (v != 0.f) {
+            c->A[s] += fabs((double)v);
+            if (c->term_val && c->nterms < c->term_cap) {
+                c->term_val[c->nterms] = v;
+                c->term_slot[c->nterms] = (int64_t)s;
+            }
+            c->nterms++;
+        }
+    }
+}
+
+/* returns the number of non-zero terms */
+long softras_oracle_backward_stats(const float *faces, const float *textures, const float *soft_colors,
+                                   const float *faces_info, const float *aggrs_info,
+                                   const int32_t *faces_id_buffer, const float *grad_soft_colors,
+                                   double *g64, double *A, int32_t *N, double *E, int batch_size,
+                                   int num_faces, int texture_size, int image_size, int max_faces_id,
+                                   float near, float far, float eps, float sigma_val, int func_id_dist,
+                                   float dist_eps, float gamma_val, int func_id_rgb, int func_id_alpha,
+                                   int texture_sample_type, int double_side, int exact_tail, int nudge,
+                                   int row_begin, int row_end, int row_stride,
+                                   float *term_val, int64_t *term_slot, long term_cap) {
+    (void)eps;
+    (void)double_side;
+    const BwdParams P = bwd_params(num_faces, texture_size, near, far, sigma_val, func_id_dist, gamma_val, func_id_rgb,
+                                   func_id_alpha, texture_sample_type);
+    const size_t ngf = (size_t)batch_size * num_faces * 9;
+    const size_t ns = ngf + (size_t)batch_size * num_faces * texture_size * 3;
+    const size_t np = 9 + 3 * (size_t)texture_size;
+    StatsCtx c = {exact_tail, nudge, ngf, g64, A, E, N, (float *)malloc(sizeof(float) * np),
+                  (float *)malloc(sizeof(float) * np), (float *)malloc(sizeof(float) * np), (float *)malloc(sizeof(float) * np),
+                  term_val, term_slot, term_cap, 0};
+    memset(g64, 0, sizeof(double) * ns);
+    memset(A, 0, sizeof(double) * ns);
+    memset(E, 0, sizeof(double) * ns);
+    memset(N, 0, sizeof(int32_t) * ns);
+    walk_pairs(faces, textures, soft_colors, faces_info, aggrs_info, faces_id_buffer, grad_soft_colors, &P, batch_size,
+               image_size, max_faces_id, dist_eps * sigma_val, row_begin, row_end, row_stride, stats_pair, &c);
+    free(c.base);
+    free(c.moved);
+    free(c.dmax);
+    free(c.dextra);
+    return c.nterms;
 }
 
 /* Multi-threaded timing variant for the CPU baseline (bench.py): thread t runs the sequential

@@ -39,6 +39,33 @@ def run_cuda(fv, tex, params, grad=None, device="cuda:0", want_faces_info=True):
     return out
 
 
+def backward_bound_ratio(got, fv, tex, params, grad, exact_tail=False, row_stride=1):
+    """Holds the SoftRas gradients of `got` (run_cuda) to the oracle's K6 sums, entry by entry.  The oracle's backward
+    runs on the kernel's own forward outputs, so both sides sum the same pairs' terms: NaN / inf must sit where the
+    oracle's do, and every finite entry meets |got - g64| <= osr.backward_bound.  exact_tail: the kernel's
+    softras_exact_tail (the bound for 0 also holds under 1).  -> {tensor: worst |got - g64| / bound}."""
+    fwd = dict(soft_colors=got["soft_colors"], aggrs_info=got["aggrs_info"], faces_id_buffer=got["faces_id_buffer"])
+    fwd["faces_info"] = got["faces_info"] if "faces_info" in got else osr.forward(fv, tex, params, rows=(0, 0))["faces_info"]
+    stats = osr.backward(fv, tex, fwd, grad, params, stats=True, exact_tail=exact_tail, row_stride=row_stride)
+    worst = {}
+    for k, st in zip(("grad_faces", "grad_textures"), stats):
+        a, ref = got[k].astype(np.float64), st["g64"]
+        assert np.array_equal(np.isnan(a), np.isnan(ref)), "%s NaN pattern differs" % k
+        assert np.array_equal(np.isposinf(a), np.isposinf(ref)) and np.array_equal(np.isneginf(a), np.isneginf(ref)), k
+        m = np.isfinite(ref)
+        err, bound = np.abs(a[m] - ref[m]), osr.backward_bound(st)[m]
+        bad = ~(err <= bound)
+        if bad.any():
+            i = np.flatnonzero(m.ravel())[np.flatnonzero(bad)]
+            j = int(i[np.argmax(err[bad] / np.maximum(bound[bad], 1e-300))])
+            idx = np.unravel_index(j, a.shape)
+            raise AssertionError("%s: %d entries outside the bound; worst at %s: got %r, oracle %r, bound %r (A %r, N %d, "
+                                 "E %r)" % (k, bad.sum(), idx, a[idx], ref[idx], osr.backward_bound(st)[idx],
+                                            st["A"][idx], st["N"][idx], st["E"][idx]))
+        worst[k] = float((err / np.maximum(bound, 1e-300)).max(initial=0.0))
+    return worst
+
+
 def sorted_ids(ids):
     """[B,K,H,W] -> per-pixel ascending id sets with -1 (empty) moved last."""
     a = ids.astype(np.int64).copy()
