@@ -222,6 +222,13 @@ B200R_API int b200r_laplacian_loss(const float* vertices, const int32_t* neighbo
  * is_update [nf] int32, textures [nf, R*R, 3] updated in place where is_update != 0.  Device pointers. */
 B200R_API int b200r_bake_textures_softras(const float* image, const float* faces_uv, const int32_t* is_update, float* textures,
                                           int nf, int texture_res, int image_height, int image_width, void* stream);
+/* The adjoint of b200r_bake_textures_softras: overwrites grad_image [H, W, 3] with the gradient of the baked textures
+ * grad_textures [nf, R*R, 3] (faces with is_update == 0 contribute nothing), scattered with the forward's bilinear weights
+ * into the pixels it read (out-of-image taps clamped to the last element, as there).  Nothing flows to faces_uv.
+ * Accumulates with float atomics, so the summation order may vary between runs.  Device pointers. */
+B200R_API int b200r_bake_textures_softras_backward(const float* grad_textures, const float* faces_uv, const int32_t* is_update,
+                                                   float* grad_image, int nf, int texture_res, int image_height,
+                                                   int image_width, void* stream);
 /* Replaces _load_textures_for_n3mr / load_textures_cuda_kernel (jrender/io/utils/load_textures.py:103-246), the bake of
  * the NMR rasterizer's [nf, ts, ts, ts, 3] textures: texel (a, b, c) samples the image at the barycentric point
  * (a, b, c) / (ts - 1) normalised to sum 1, through the face's wrapped UVs.  texture_wrapping: 0 REPEAT, 1 MIRRORED_REPEAT,
@@ -359,7 +366,8 @@ B200R_API int b200r_vol_resample(const float* z_vals, const float* bins, const f
  * Replaces the map stages of SSS (jrender/renderer/lighting/lighting.py:108-150): computeStretchMap
  * (renderer/utils/ToStretchMap.py:5-13) and the gaussian_blur / _blur_for_SSS ops (renderer/utils/gaussian_blur.py:4-204).
  * Maps are float32 device planes [H, W], row 0 = the top row of the SoftRas image they were rasterized into; [3, H, W]
- * inputs are planar (the first three planes of a SoftRas soft_colors [4, H, W] can be passed as they are).  No gradient.
+ * inputs are planar (the first three planes of a SoftRas soft_colors [4, H, W] can be passed as they are).  Gradients: the
+ * _backward entry points below.
  *   b200r_sss_stretch: world_map [3, H, W] (world coordinates, before the reference's `* 7`) -> stretch_u, stretch_v
  *       [H, W]: 1 / |7 (w(y, x) - w(y, x + 1))| and 1 / |7 (w(y, x) - w(y + 1, x))| with the last column / row replicated,
  *       each clamped to [0, 1].  One launch.
@@ -377,6 +385,27 @@ B200R_API int b200r_sss_blur_pyramid(const float* stretch_u, const float* stretc
                                      const float* specular_map, float* out_map, void* workspace, size_t workspace_bytes,
                                      const float* taps, const float* tap_widths, const float* weights, int num_levels,
                                      int height, int width, void* stream);
+/* Gradients (Lighting.sss_grad):
+ *   b200r_sss_stretch_backward: overwrites grad_world_map [3, H, W] with the gradient of world_map through
+ *       b200r_sss_stretch, given grad_stretch_u / grad_stretch_v [H, W].  Where a clamp is active (including every
+ *       face's inside, where the difference is 0) the gradient is 0.  No atomics; one launch.
+ *   b200r_sss_blur_pyramid_backward: given the forward's inputs stretch_u, stretch_v, irradiance_map [3, H, W] and
+ *       grad_out [H, W, 3] (rows flipped, as out_map), overwrites grad_irradiance_map and grad_specular_map [3, H, W], and,
+ *       when both are non-NULL, grad_stretch_u / grad_stretch_v [H, W] (both NULL: the stretch maps' gradients and their
+ *       modulation terms are not computed).  The gradients are taken at the forward's decisions (tap indices, clamps,
+ *       the <= 1e-6 replacements and the centre test).  Same taps, tap_widths, weights, num_levels and square-map rule
+ *       as the forward, and width <= 8192.  workspace: b200r_sss_backward_workspace_bytes(H, W, num_levels) bytes
+ *       ((8 num_levels + 10) maps; 0 for out-of-range arguments), else B200R_EWORKSPACE.  The forward's 2 * num_levels
+ *       launches again, then 2 * num_levels backward launches; y-pass gradients are summed with float atomics, so the
+ *       order of the sums may vary between runs. */
+B200R_API size_t b200r_sss_backward_workspace_bytes(int height, int width, int num_levels);
+B200R_API int b200r_sss_stretch_backward(const float* world_map, const float* grad_stretch_u, const float* grad_stretch_v,
+                                         float* grad_world_map, int height, int width, void* stream);
+B200R_API int b200r_sss_blur_pyramid_backward(const float* stretch_u, const float* stretch_v, const float* irradiance_map,
+                                              const float* grad_out, float* grad_irradiance_map, float* grad_specular_map,
+                                              float* grad_stretch_u, float* grad_stretch_v, void* workspace,
+                                              size_t workspace_bytes, const float* taps, const float* tap_widths,
+                                              const float* weights, int num_levels, int height, int width, void* stream);
 
 /* Launch counter: number of kernels this library has launched in this process
  * (bench.py reports the delta over the timed region as "gpu_launches"). */

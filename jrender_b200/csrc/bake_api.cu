@@ -53,6 +53,43 @@ k_bake_textures_softras(const float* __restrict__ image, const float* __restrict
     }
 }
 
+// Adjoint of k_bake_textures_softras: every texel of a face with is_update != 0 adds its gradient times the forward's
+// four bilinear weights (same promotions) into the same clamped pixels the forward read.  grad_image is zeroed first.
+__global__ void __launch_bounds__(256)
+k_bake_textures_softras_bwd(const float* __restrict__ grad_textures, const float* __restrict__ faces_uv,
+                            const int32_t* __restrict__ is_update, float* __restrict__ grad_image, long ntexels, int R, int H,
+                            int W) {
+    const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= ntexels) return;
+    const int fn = (int)(i / (R * R));
+    if (__ldg(is_update + fn) == 0) return;
+    const int w_y = (int)(i % (R * R)) / R, w_x = (int)(i % R);
+    float w0, w1, w2;
+    if (w_x + w_y < R) {
+        w0 = (float)((w_x + 1. / 3.) / R);
+        w1 = (float)((w_y + 1. / 3.) / R);
+    } else {
+        w0 = (float)(((R - 1. - w_x) + 2. / 3.) / R);
+        w1 = (float)(((R - 1. - w_y) + 2. / 3.) / R);
+    }
+    w2 = (float)(1. - (double)w0 - (double)w1);
+    const float* face = faces_uv + (size_t)fn * 6;
+    const float pos_x = (__ldg(face + 0) * w0 + __ldg(face + 2) * w1 + __ldg(face + 4) * w2) * (float)(W - 1);
+    const float pos_y = (__ldg(face + 1) * w0 + __ldg(face + 3) * w1 + __ldg(face + 5) * w2) * (float)(H - 1);
+    const float weight_x1 = pos_x - (int)pos_x, weight_x0 = 1 - weight_x1;
+    const float weight_y1 = pos_y - (int)pos_y, weight_y0 = 1 - weight_y1;
+    const long n = (long)H * W;
+    const long i00 = (long)(int)pos_y * W + (int)pos_x, i10 = (long)(int)(pos_y + 1) * W + (int)pos_x;
+    const long idx[4] = {i00, i10, i00 + 1, i10 + 1};
+    const float wt[4] = {weight_x0 * weight_y0, weight_x0 * weight_y1, weight_x1 * weight_y0, weight_x1 * weight_y1};
+#pragma unroll
+    for (int k = 0; k < 3; k++) {
+        const float g = __ldg(grad_textures + i * 3 + k);
+#pragma unroll
+        for (int j = 0; j < 4; j++) atomicAdd(grad_image + (idx[j] < 0 ? 0 : (idx[j] >= n ? n - 1 : idx[j])) * 3 + k, g * wt[j]);
+    }
+}
+
 // fmod-based wrap of the reference (:112-119): x > 0 -> fmod(x, y), else y + fmod(x, y)
 __device__ __forceinline__ float ref_mod(float x, float y) { return x > 0.f ? fmodf(x, y) : y + fmodf(x, y); }
 
@@ -148,4 +185,21 @@ extern "C" int b200r_bake_textures_softras(const float* image, const float* face
     const long ntexels = (long)nf * texture_res * texture_res;
     return b200r_launch("k_bake_textures_softras", B200R_K_BAKE, k_bake_textures_softras, (unsigned)((ntexels + 255) / 256), 256, 0, st,
                         image, faces_uv, is_update, textures, ntexels, texture_res, image_height, image_width);
+}
+
+extern "C" int b200r_bake_textures_softras_backward(const float* grad_textures, const float* faces_uv, const int32_t* is_update,
+                                                    float* grad_image, int nf, int texture_res, int image_height,
+                                                    int image_width, void* stream) {
+    if (!grad_textures || !faces_uv || !is_update || !grad_image)
+        return b200r_fail(B200R_EINVAL, "b200r_bake_textures_softras_backward: NULL pointer argument");
+    if (nf <= 0 || texture_res <= 0 || image_height <= 0 || image_width <= 0)
+        return b200r_fail(B200R_EINVAL, "b200r_bake_textures_softras_backward: non-positive size");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (int rc = b200r_zero(grad_image, (size_t)image_height * image_width * 3 * sizeof(float), st,
+                            "b200r_bake_textures_softras_backward"))
+        return rc;
+    const long ntexels = (long)nf * texture_res * texture_res;
+    return b200r_launch("k_bake_textures_softras_bwd", B200R_K_BAKE, k_bake_textures_softras_bwd,
+                        (unsigned)((ntexels + 255) / 256), 256, 0, st, grad_textures, faces_uv, is_update, grad_image, ntexels,
+                        texture_res, image_height, image_width);
 }

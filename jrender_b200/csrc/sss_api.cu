@@ -27,27 +27,11 @@
 
 #include "../../include/b200raster.h"
 #include "api_util.cuh"
+#include "sss_common.cuh"
 
 namespace {
 
-constexpr int kTaps = 7;              // tap_num, lighting.py:117
-constexpr int kMaxLevels = 8;
-constexpr int kBlockX = 32, kBlockY = 8;
-
-struct SssPass {
-    const float* s_in;      // stretch map of the previous level [H, W]
-    float* s_out;           // this level's blurred stretch map, or NULL (last level: nobody reads it)
-    const float* irr_in;    // [3, H, W]
-    float* irr_out;         // [3, H, W], or NULL (last y pass)
-    float* acc;             // y passes: [3, H, W] running weighted sum of the levels
-    const float* irr0;      // last y pass: the unblurred irradiance map [3, H, W]
-    const float* spec;      // last y pass: the specular map [3, H, W]
-    float* out;             // last y pass: [H, W, 3], rows flipped
-    float taps[kTaps];
-    float width;            // GaussWidth = float32(sqrt(v))
-    float weight[3];        // y passes: this level's weight per channel
-    int H, W, first, last;
-};
+using namespace b200r_sss;
 
 // One blurred value of gaussain_blur_{x,y}_Kernel (gaussian_blur.py:43-97, 109-164) for a single-channel map: `p` points
 // at the line through the pixel (its row for x, its column for y, `stride` apart), `c` is the pixel's index on that line
@@ -148,6 +132,11 @@ __global__ void __launch_bounds__(kBlockX * kBlockY) k_sss_blur_y(const SssPass 
 constexpr int kPlanes = 13;
 
 }  // namespace
+
+void b200r_sss::forward_kernels(PassKernel* x_pass, PassKernel* y_pass) {
+    *x_pass = k_sss_blur_x;
+    *y_pass = k_sss_blur_y;
+}
 
 extern "C" size_t b200r_sss_workspace_bytes(int height, int width) {
     if (height <= 0 || width <= 0) return 0;

@@ -263,7 +263,99 @@ def _sss_maps(diffuseLight, specular, mesh):
     return world_map, irradiance_map, specular_map
 
 
-def SSS(diffuseLight, specular, mesh):
+def _sss_levels():
+    """The host arrays of the blur pyramid: (taps [L][7], tap widths [L], weights [3][L], L) as ctypes float arrays."""
+    variances = [SSS_GAUSSIAN_BASIS[i + 1] - SSS_GAUSSIAN_BASIS[i] for i in range(len(SSS_GAUSSIAN_BASIS) - 1)]
+    L = len(variances)
+    taps, widths = zip(*[_sss_taps(v) for v in variances])
+    return ((C.c_float * (L * SSS_TAP_NUM))(*[t for level in taps for t in level]), (C.c_float * L)(*widths),
+            (C.c_float * (3 * L))(*[w for channel in SSS_WEIGHTS for w in channel]), L)
+
+
+def _map_grad(like):
+    """A gradient for a [1, 4, S, S] SoftRas map whose first three planes a kernel overwrites: the alpha plane is 0."""
+    g = torch.empty_like(like)
+    g[:, 3].zero_()
+    return g
+
+
+class _SSSStretch(torch.autograd.Function):
+    """b200r_sss_stretch / _backward: the world-coordinate map [1, 4, S, S] -> the clamped stretch maps (u, v) [S, S]."""
+
+    @staticmethod
+    def forward(ctx, world_map):
+        S = world_map.shape[-1]
+        su = torch.empty((S, S), dtype=torch.float32, device=world_map.device)
+        sv = torch.empty_like(su)
+        _lib.call("b200r_sss_stretch", world_map.device, world_map, su, sv, S, S)
+        ctx.save_for_backward(world_map)
+        return su, sv
+
+    @staticmethod
+    def backward(ctx, gu, gv):
+        world_map, = ctx.saved_tensors
+        S = world_map.shape[-1]
+        gw = _map_grad(world_map)
+        _lib.call("b200r_sss_stretch_backward", world_map.device, world_map, gu.contiguous(), gv.contiguous(), gw, S, S)
+        return gw
+
+
+class _SSSPyramid(torch.autograd.Function):
+    """b200r_sss_blur_pyramid / _backward: (stretch u, v [S, S], irradiance and specular maps [1, 4, S, S]) -> the
+    composed map [S, S, 3], rows flipped."""
+
+    @staticmethod
+    def forward(ctx, stretch_u, stretch_v, irradiance_map, specular_map):
+        dev, S = stretch_u.device, stretch_u.shape[-1]
+        taps, widths, weights, L = _sss_levels()
+        nbytes = _lib.lib().b200r_sss_workspace_bytes(S, S)
+        workspace = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+        final_map = torch.empty((S, S, 3), dtype=torch.float32, device=dev)
+        _lib.call("b200r_sss_blur_pyramid", dev, stretch_u, stretch_v, irradiance_map, specular_map, final_map, workspace,
+                  nbytes, taps, widths, weights, L, S, S)
+        ctx.save_for_backward(stretch_u, stretch_v, irradiance_map)
+        return final_map
+
+    @staticmethod
+    def backward(ctx, g):
+        su, sv, irr = ctx.saved_tensors
+        dev, S = su.device, su.shape[-1]
+        taps, widths, weights, L = _sss_levels()
+        stretch = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+        gsu = torch.empty_like(su) if stretch else None
+        gsv = torch.empty_like(sv) if stretch else None
+        girr, gspec = _map_grad(irr), _map_grad(irr)
+        nbytes = _lib.lib().b200r_sss_backward_workspace_bytes(S, S, L)
+        workspace = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
+        _lib.call("b200r_sss_blur_pyramid_backward", dev, su, sv, irr, g.contiguous(), girr, gspec, gsu, gsv, workspace,
+                  nbytes, taps, widths, weights, L, S, S)
+        return gsu, gsv, girr, gspec
+
+
+class _SSSBake(torch.autograd.Function):
+    """b200r_bake_textures_softras / _backward on the composed map [S, S, 3]: every face's R*R texels, [nf, R*R, 3]."""
+
+    @staticmethod
+    def forward(ctx, final_map, faces_uv, R):
+        dev, nf = final_map.device, faces_uv.shape[0]
+        upd = torch.ones((nf,), dtype=torch.int32, device=dev)
+        out = torch.ones((nf, R * R, 3), dtype=torch.float32, device=dev)
+        _lib.call("b200r_bake_textures_softras", dev, final_map, faces_uv, upd, out, nf, R, final_map.shape[0],
+                  final_map.shape[1])
+        ctx.save_for_backward(faces_uv, upd)
+        ctx.R, ctx.shape = R, final_map.shape
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        faces_uv, upd = ctx.saved_tensors
+        gmap = torch.empty(ctx.shape, dtype=torch.float32, device=g.device)
+        _lib.call("b200r_bake_textures_softras_backward", g.device, g.contiguous(), faces_uv, upd, gmap, faces_uv.shape[0],
+                  ctx.R, ctx.shape[0], ctx.shape[1])
+        return gmap, None, None
+
+
+def SSS(diffuseLight, specular, mesh, grad=False):
     """Texture-space subsurface scattering, lighting.py:86-156: the mesh's textures [1, nf, R*R, 3] lit by diffuseLight
     and specular ([1, nf, 1, 3] per face, or [1, nf, R*R, 3] per texel), returned as new textures [1, nf, R*R, 3]
     (unclamped; Lighting clamps them).
@@ -273,8 +365,15 @@ def SSS(diffuseLight, specular, mesh):
     coordinate map into the clamped stretch maps; b200r_sss_blur_pyramid blurs the irradiance over three levels, modulated
     by the stretch, and composes `sum_k w_k blur_k * irradiance + specular`; the bake samples that map back into textures.
 
-    As in the reference, gradients stop here: the result does not require grad.  The batch must be 1, the mesh must carry
-    face_texcoords, and its textures must hold texture_res^2 texels per face (ValueError otherwise)."""
+    With grad=False (the default), as in the reference, gradients stop here: the result does not require grad.  With
+    grad=True and grad mode on, the result carries a graph to textures, diffuseLight, specular and the mesh's
+    face_vertices (through the world-coordinate and stretch maps), through the backward kernels of each stage and the
+    SoftRas backward of the three texture-space rasterizations; the values are the same bits either way.  The gradient
+    of sqrt(textures * diffuse) is infinite where the product is 0, as torch's own: keep fitted textures away from 0.
+    Nothing flows to face_texcoords, which must not require grad then (ValueError).
+
+    The batch must be 1, the mesh must carry face_texcoords, and its textures must hold texture_res^2 texels per face
+    (ValueError otherwise)."""
     from . import io
     tx = mesh.textures
     if tx.dim() != 4 or tx.shape[0] != 1:
@@ -290,17 +389,20 @@ def SSS(diffuseLight, specular, mesh):
         raise ValueError("SSS: face_texcoords %s do not match %d faces" % (tuple(ftc.shape), nf))
     dev = tx.device
     S = SSS_IMAGE_SIZE
+    if grad and torch.is_grad_enabled():
+        if ftc.requires_grad:
+            raise ValueError("SSS: face_texcoords require grad, but no gradient flows to them")
+        if any(t.requires_grad for t in (diffuseLight, specular, tx, mesh.face_vertices)):
+            world_map, irradiance_map, specular_map = _sss_maps(diffuseLight, specular, mesh)
+            stretch_u, stretch_v = _SSSStretch.apply(world_map)
+            final_map = _SSSPyramid.apply(stretch_u, stretch_v, irradiance_map, specular_map)
+            return _SSSBake.apply(final_map, ftc[0].to(dev, torch.float32).contiguous(), R)[None]
     with torch.no_grad():
         world_map, irradiance_map, specular_map = _sss_maps(diffuseLight, specular, mesh)
         stretch_u = torch.empty((S, S), dtype=torch.float32, device=dev)
         stretch_v = torch.empty_like(stretch_u)
         _lib.call("b200r_sss_stretch", dev, world_map, stretch_u, stretch_v, S, S)
-        variances = [SSS_GAUSSIAN_BASIS[i + 1] - SSS_GAUSSIAN_BASIS[i] for i in range(len(SSS_GAUSSIAN_BASIS) - 1)]
-        L = len(variances)
-        taps, widths = zip(*[_sss_taps(v) for v in variances])
-        taps = (C.c_float * (L * SSS_TAP_NUM))(*[t for level in taps for t in level])
-        widths = (C.c_float * L)(*widths)
-        weights = (C.c_float * (3 * L))(*[w for channel in SSS_WEIGHTS for w in channel])
+        taps, widths, weights, L = _sss_levels()
         nbytes = _lib.lib().b200r_sss_workspace_bytes(S, S)
         workspace = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
         final_map = torch.empty((S, S, 3), dtype=torch.float32, device=dev)
@@ -358,6 +460,7 @@ class Lighting(nn.Module):
         self.directionals = nn.ModuleList([DirectionalLighting(intensity_directionals, color_directionals, directions)])
 
     fused = True   # CUDA float32 surface-mode inputs take the one-launch kernel (b200r_surface_lighting_forward)
+    sss_grad = False   # with_SSS meshes: differentiate SSS (SSS(..., grad=True)); off, its result carries no graph
 
     def _fusable(self, mesh, eyes):
         tx, v = mesh.textures, mesh.vertices
@@ -475,7 +578,7 @@ class Lighting(nn.Module):
                     mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
             diffuseLight = diffuseLight[:, :, None, :]
             specularLight = specularLight[:, :, None, :]
-        mesh.textures = torch.clamp(SSS(diffuseLight, specularLight, mesh), 0.0, 1.0)
+        mesh.textures = torch.clamp(SSS(diffuseLight, specularLight, mesh, grad=self.sss_grad), 0.0, 1.0)
         return mesh
 
     def forward(self, mesh, eyes=None):

@@ -126,3 +126,22 @@ def nmr_scene(num_faces=280, batch=1, ts=2, fill_back=True, seed=1):
         fv = np.concatenate([fv, fv[:, :, ::-1]], axis=1)
         tex = np.concatenate([tex, tex.transpose(0, 1, 4, 3, 2, 5)], axis=1)
     return np.ascontiguousarray(fv), np.ascontiguousarray(tex)
+
+
+def sss_maps(size, seed):
+    """Synthetic texture-space SSS maps [size, size, 3] (size a multiple of 16): (world, irradiance, specular).  The
+    world coordinates are flat over 16 x 16 patches, as rasterized world coordinates are flat over faces, and some
+    patches vary along x, so that the stretch takes values inside (0, 1); all three are zero in background holes."""
+    rng = np.random.default_rng(seed)
+    n = size // 16
+    world = np.kron(rng.uniform(0, 255, (n, n, 3)), np.ones((16, 16, 1))).astype(np.float32)
+    world += np.kron(rng.uniform(0, 1, (n, n, 1)), np.ones((16, 16, 3))).astype(np.float32) * np.float32(0.02) \
+        * np.arange(size, dtype=np.float32)[None, :, None]
+    hole = np.kron(rng.random((n, n)) < 0.3, np.ones((16, 16))).astype(bool)
+    hole[:5] = True
+    hole[:, -7:] = True
+    irr = rng.uniform(0, 1, (size, size, 3)).astype(np.float32)
+    spec = rng.uniform(0, 0.3, (size, size, 3)).astype(np.float32)
+    for a in (world, irr, spec):
+        a[hole] = 0
+    return world, irr, spec
