@@ -48,10 +48,15 @@ class LaplacianLoss(nn.Module):
         self.nf = faces.shape[0]
         self.average = average
         f = faces.detach().cpu().numpy().astype(np.int64)
-        # off-diagonal -1 for every (undirected) edge, diagonal = degree, rows divided by the diagonal
+        # laplacian_loss.py:14-27: -1 at (i, j) for every (undirected) edge, diagonal = minus the row sum, rows divided
+        # by the diagonal.  A face with a repeated index writes -1 at (a, a) first, which the diagonal then overwrites:
+        # the self-pair adds 1 to the divisor but a is not its own neighbour.
         e = np.concatenate([f[:, [0, 1]], f[:, [1, 0]], f[:, [1, 2]], f[:, [2, 1]], f[:, [2, 0]], f[:, [0, 2]]], 0)
         e = np.unique(e, axis=0)
-        deg = np.bincount(e[:, 0], minlength=self.nv).astype(np.float32)
+        self_pair = e[:, 0] == e[:, 1]
+        div = np.bincount(e[:, 0], minlength=self.nv).astype(np.float32)   # distinct neighbours + has a self-pair
+        e = e[~self_pair]
+        deg = np.bincount(e[:, 0], minlength=self.nv)
         # Padded neighbour table instead of a sparse matrix: L x = diag * x + sum_k w[:, k] * x[nbr[:, k]].
         # index_select forward / index_add backward are plain kernels (no thrust sort, no host
         # synchronisation), so the loss can be captured in a CUDA graph; torch.sparse.mm cannot.
@@ -61,10 +66,10 @@ class LaplacianLoss(nn.Module):
         fill = np.zeros(self.nv, np.int64)
         for a_, b_ in e:
             nbr[a_, fill[a_]] = b_
-            w[a_, fill[a_]] = -1.0 / deg[a_]
+            w[a_, fill[a_]] = -1.0 / div[a_]
             fill[a_] += 1
         with np.errstate(divide='ignore', invalid='ignore'):
-            diag = (deg / deg).astype(np.float32)     # 1, or NaN for an isolated vertex like the dense 0/0
+            diag = (div / div).astype(np.float32)     # 1, or NaN for an isolated vertex like the dense 0/0
         self.register_buffer('nbr', torch.from_numpy(nbr.reshape(-1)))
         self.register_buffer('nbr32', torch.from_numpy(nbr.astype(np.int32)))
         self.register_buffer('nbr_w', torch.from_numpy(w))
@@ -95,6 +100,11 @@ class FlattenLoss(nn.Module):
         self.average = average
         f = faces.detach().cpu().numpy().astype(np.int64)
         self.nv_min = int(f.max()) + 1 if f.size else 0   # smallest vertex count the edge table is valid for
+        # a face with a repeated index has an edge with no third vertex (flatten_loss.py:22-24 raises IndexError on it);
+        # the table below would pair that face with itself instead
+        rep = np.flatnonzero((f[:, 0] == f[:, 1]) | (f[:, 1] == f[:, 2]) | (f[:, 2] == f[:, 0]))
+        if rep.size:
+            raise ValueError("FlattenLoss: face %d %s repeats a vertex index" % (rep[0], f[rep[0]].tolist()))
         opp = {}
         for tri in f:
             for a, b_, c in ((tri[0], tri[1], tri[2]), (tri[1], tri[2], tri[0]), (tri[2], tri[0], tri[1])):

@@ -33,7 +33,8 @@ class Mesh(object):
         if isinstance(vertices, np.ndarray):
             vertices = torch.from_numpy(vertices).float()
         if isinstance(faces, np.ndarray):
-            faces = torch.from_numpy(faces).int()
+            from .preraster import int32_faces
+            faces = int32_faces(torch.from_numpy(np.asarray(faces, np.int64)), 'cpu')
         self._vertices = vertices
         self._faces = faces
         self._projector = None

@@ -56,11 +56,16 @@ class _ProjectFacesOp(torch.autograd.Function):
         return gv, None, None, None
 
 
-def _int32_faces(faces, dev):
+def int32_faces(faces, dev):
     """int32 + contiguous, no host synchronisation: the kernel range-checks every index itself (an
-    index outside [0, nv) poisons that corner with NaN instead of the reference's out-of-bounds read)."""
-    f = faces if faces.dtype == torch.int32 else faces.to(torch.int32)
-    return f.to(dev).contiguous()
+    index outside [0, nv) poisons that corner with NaN instead of the reference's out-of-bounds read).
+    Wider indices outside [0, 2^31) become -1 on the device first: a plain cast would wrap 2^32 + 1 to 1."""
+    f = faces.to(dev)
+    if f.dtype != torch.int32:
+        if f.dtype == torch.int64:
+            f = f.masked_fill((f < 0) | (f > 0x7fffffff), -1)
+        f = f.to(torch.int32)
+    return f.contiguous()
 
 
 def project_faces(vertices, faces, eye, camera_mode='look_at', at=(0, 0, 0), direction=(0, 0, 1), up=(0, 1, 0),
@@ -92,7 +97,7 @@ def project_faces(vertices, faces, eye, camera_mode='look_at', at=(0, 0, 0), dir
             raise ValueError("%s batch %d does not match batch size %d" % (name, t.shape[0], B))
     if e.shape[1:] != (3,):
         raise ValueError("eye must be [3] or [batch, 3]")
-    f = _int32_faces(faces, dev)
+    f = int32_faces(faces, dev)
     if camera_mode == 'look_at':
         mode, a = CAM_MODES['look_at'], _f3(at)
     elif camera_mode == 'look':

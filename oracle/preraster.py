@@ -80,8 +80,87 @@ def project_faces(vertices, faces, eye, camera_mode="look_at", at=(0, 0, 0), dir
     faces = np.broadcast_to(faces, (B,) + faces.shape[1:])
     eye = np.broadcast_to(eye, (B, 3))
     r = camera_axes(eye, camera_mode, at, direction, up, coordinate)
-    pv = project(to_camera(vertices, eye, r), perspective, viewing_angle, viewing_scale)
-    return np.stack([pv[b][faces[b].astype(np.int64)] for b in range(B)], axis=0).astype(F)   # faces_vertices.py:16-19
+    with np.errstate(all="ignore"):
+        pv = project(to_camera(vertices, eye, r), perspective, viewing_angle, viewing_scale)
+    nv = pv.shape[1]
+    idx = faces.astype(np.int64)
+    bad = (idx < 0) | (idx >= nv)   # the kernel poisons such a corner instead of the reference's out-of-bounds read
+    out = np.stack([pv[b][np.where(bad[b], 0, idx[b])] for b in range(B)], axis=0).astype(F)   # faces_vertices.py:16-19
+    out[bad] = np.nan
+    return out
+
+
+def project_faces_bwd_terms(vertices, faces, eye, grad_face_vertices, lift=None, camera_mode="look_at", at=(0, 0, 0),
+                            direction=(0, 0, 1), up=(0, 1, 0), coordinate="right", perspective=True, viewing_angle=30.0,
+                            viewing_scale=1.0):
+    """k_project_faces_bwd's contribution of every (image, face, corner) to grad_vertices, in the kernel's float32 order:
+    cam = (v - eye) r^T; zw = Z*w, dc0 = gx/zw, dc1 = gy/zw, dc2 = gz - (gx*X + gy*Y)/(Z*zw) (orthogonal: gx*s, gy*s, gz);
+    term_k = (dc0*r0k + dc1*r1k) + dc2*r2k.  Corners with an out-of-range index or an all-zero upstream gradient add
+    nothing, as in the kernel.  -> (rows [n], terms = three arrays [n], one per coordinate k): rows index
+    grad_vertices.reshape(-1, 3), one per contributing corner.
+    `lift` maps every float32 input array to another number type that supports the same operators (identity: float32)."""
+    v = np.asarray(vertices, F)
+    Bv, nv = v.shape[:2]
+    g = np.asarray(grad_face_vertices, F)
+    B, nf = g.shape[:2]
+    f = np.broadcast_to(np.asarray(faces).astype(np.int64), (B, nf, 3)).reshape(-1)
+    e = np.broadcast_to(np.asarray(eye, F).reshape(-1, 3), (B, 3))
+    r = camera_axes(e, camera_mode, at, direction, up, coordinate)
+    b = np.repeat(np.arange(B), nf * 3)
+    gg = g.reshape(-1, 3)
+    keep = (f >= 0) & (f < nv) & (gg != 0).any(1)
+    b, f, gg = b[keep], f[keep], gg[keep]
+    rows = (b if Bv > 1 else 0) * nv + f
+    lift = lift or (lambda x: x)
+    vv, ee, rr, G = lift(v.reshape(-1, 3)[rows]), lift(e[b]), lift(r[b]), lift(gg)
+    with np.errstate(all="ignore"):
+        d = [vv[:, k] - ee[:, k] for k in range(3)]
+        cam = [(d[0] * rr[:, i, 0] + d[1] * rr[:, i, 1]) + d[2] * rr[:, i, 2] for i in range(3)]
+        gx, gy, gz = G[:, 0], G[:, 1], G[:, 2]
+        if perspective:
+            zw = cam[2] * perspective_width(viewing_angle)
+            dc = [gx / zw, gy / zw, gz - (gx * cam[0] + gy * cam[1]) / (cam[2] * zw)]
+        else:
+            s = F(viewing_scale)
+            dc = [gx * s, gy * s, gz]
+        terms = [(dc[0] * rr[:, 0, k] + dc[1] * rr[:, 1, k]) + dc[2] * rr[:, 2, k] for k in range(3)]
+    return rows, terms
+
+
+U = 2.0 ** -24      # fp32 unit roundoff
+FTZ = 2.0 ** -125   # the float atomics flush subnormal inputs and results: < 2^-126 lost on each, per add
+
+
+def term_sums(slots, terms, size):
+    """Entries a kernel accumulates from float32 `terms` (one per slot, in [0, size)) in an unspecified order: warp
+    shuffles, block partial sums and float atomics, all trees of float additions starting from zero.  Returns dict of
+    float64 arrays of length `size`:
+        exact  the sum of the terms (float64, within n 2^-53 A of the exact sum),
+        A      sum of |t|,  n  the number of terms,
+        bound  gamma_{n-1} A + n 2^-52 A + n 2^-125,  gamma_k = k u / (1 - k u),  u = 2^-24:
+    any order of float additions is within gamma_{n-1} A of the exact sum (Higham, Accuracy and Stability of Numerical
+    Algorithms, 4.2); the second term covers the float64 sum's own error, the third the atomics' subnormal flush.
+    Entries whose exact sum is not finite are not bounded: their NaN / +-inf pattern does not depend on the order."""
+    slots = np.asarray(slots, np.int64).reshape(-1)
+    t = np.asarray(terms, np.float64).reshape(-1)
+    exact, A = np.zeros(size), np.zeros(size)
+    with np.errstate(invalid="ignore"):
+        np.add.at(exact, slots, t)
+        np.add.at(A, slots, np.abs(t))
+    n = np.bincount(slots, minlength=size).astype(np.float64)
+    k = np.maximum(n - 1, 0)
+    with np.errstate(invalid="ignore"):
+        bound = k * U / (1 - k * U) * A + n * 2.0 ** -52 * A + n * FTZ
+    return dict(exact=exact, A=A, n=n, bound=bound)
+
+
+def project_faces_bwd_sums(vertices, faces, eye, grad_face_vertices, **kw):
+    """term_sums of k_project_faces_bwd's corner terms, each array shaped like grad_vertices [Bv, nv, 3]."""
+    rows, terms = project_faces_bwd_terms(vertices, faces, eye, grad_face_vertices, **kw)
+    shape = np.shape(vertices)
+    slots = rows[:, None] * 3 + np.arange(3)
+    s = term_sums(slots, np.stack(terms, 1), int(np.prod(shape)))
+    return {k: x.reshape(shape) for k, x in s.items()}
 
 
 def project_faces_vjp(vertices, faces, eye, grad_face_vertices, vertices_batch=None, **kw):

@@ -1,6 +1,7 @@
 """GPU parity of the fused mesh regularisers (csrc/mesh_loss_api.cu, SURVEY.md 8f rank 4): value and
 gradient against the op-by-op PyTorch mirror (itself pinned to the reference's Python by
-tests/test_host_golden.py) and against the reference-Python golden values directly."""
+tests/test_host_golden.py), against the reference-Python golden values directly, against central differences of the
+float64 oracle, and every entry within the summation-order bound of the oracle's emulated float32 terms."""
 import os
 
 import numpy as np
@@ -46,8 +47,11 @@ def test_fused_losses_match_mirror_and_golden(which, cuda_device):
 @pytest.mark.parametrize("which", ["laplacian", "flatten", "flatten_rot"])
 def test_fused_loss_gradients_against_numeric_oracle(which, cuda_device):
     """Gradients of the fused kernels against oracle/mesh_loss.py: float64 restatement of the reference's expressions,
-    differentiated by central differences (independent of the PyTorch mirror and of any autograd)."""
+    differentiated by central differences (independent of the PyTorch mirror and of any autograd); and every value and
+    gradient entry within the summation-order bound of the oracle's float32 emulation of the kernels' terms (the
+    emulation is held to float64 in test_geometry_edges_cpu.py)."""
     from oracle import mesh_loss as oml
+    from tests.geometry_edge_cases import check_sums
     g = np.load(os.path.join(G, "ref_host_loss_sphere280.npz"))
     vb = g["vertices"]
     faces = g["faces_rot"] if which == "flatten_rot" else g["faces"]
@@ -56,12 +60,19 @@ def test_fused_loss_gradients_against_numeric_oracle(which, cuda_device):
         mod = jr.LaplacianLoss(torch.from_numpy(vb[0]), f)
         lap = oml.laplacian_matrix(vb.shape[1], faces)
         fn = lambda x: oml.laplacian(x, lap)                      # noqa: E731
+        s = oml.laplacian_sums(vb, mod.nbr32.numpy(), mod.nbr_w.numpy(), mod.diag.numpy())
     else:
         mod = jr.FlattenLoss(f)
         edges = oml.flatten_edges(faces)
         fn = lambda x: oml.flatten(x, edges)                      # noqa: E731
+        s = oml.flatten_sums(vb, edges)
     mod = mod.to(cuda_device)
     v = torch.from_numpy(vb).to(cuda_device).requires_grad_(True)
+    val = mod(v)
+    val.sum().backward()     # an upstream gradient of 1 leaves the kernel's gradient unrounded
+    check_sums(which + " loss", val.detach().cpu().numpy(), s["loss"])
+    check_sums(which + " grad", v.grad.cpu().numpy(), s["grad"])
+    v.grad = None
     val = mod(v)
     w = np.linspace(0.5, 1.5, val.numel())
     (val * torch.from_numpy(w.astype(np.float32)).to(cuda_device)).sum().backward()
