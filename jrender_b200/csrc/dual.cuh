@@ -97,12 +97,20 @@ __device__ __forceinline__ Dual<N> dsqrt(const Dual<N>& a) {
     for (int i = 0; i < N; i++) r.d[i] = a.d[i] * h;
     return r;
 }
-// max(a, lo): gradient passes where a > lo (torch.relu / clamp(min=) convention: 0 at the kink for relu).  NaN
-// propagates as torch.relu / clamp do: the value stays NaN and its derivative is 0 (the mask `a > lo` is false).
+// max(a, lo) as torch.relu: the derivative passes where a > lo, not at the kink (relu'(0) = 0).  NaN propagates as
+// torch does: the value stays NaN and its derivative is 0 (the mask `a > lo` is false).
 __device__ __forceinline__ float dmax(float a, float lo) { return a <= lo ? lo : a; }
 template <int N>
 __device__ __forceinline__ Dual<N> dmax(const Dual<N>& a, float lo) {
     if (a.v > lo) return a;
+    return dconst<N>(a.v <= lo ? lo : a.v);
+}
+// max(a, lo) as torch.clamp(min=lo) / clamp_min (and so F.normalize's eps): the derivative passes where a >= lo,
+// at equality included.  NaN as in dmax: value NaN, derivative 0.
+__device__ __forceinline__ float dclamp_min(float a, float lo) { return a <= lo ? lo : a; }
+template <int N>
+__device__ __forceinline__ Dual<N> dclamp_min(const Dual<N>& a, float lo) {
+    if (a.v >= lo) return a;
     return dconst<N>(a.v <= lo ? lo : a.v);
 }
 __device__ __forceinline__ float dvalue(float a) { return a; }

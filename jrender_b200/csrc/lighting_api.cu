@@ -50,10 +50,10 @@ __device__ __forceinline__ S dot3(const S a[3], const S b[3]) { return a[0] * b[
 template <class S>
 __device__ __forceinline__ S dot3f(const S a[3], const float b[3]) { return a[0] * b[0] + a[1] * b[1] + a[2] * b[2]; }
 
-// x / max(||x||, eps)   (F.normalize / jt.normalize)
+// x / max(||x||, eps)   (F.normalize / jt.normalize: clamp_min, so the norm's derivative passes at ||x|| == eps)
 template <class S>
 __device__ __forceinline__ void normalize3(S x[3], float eps) {
-    const S n = dmax(dsqrt(dot3(x, x)), eps);
+    const S n = dclamp_min(dsqrt(dot3(x, x)), eps);
 #pragma unroll
     for (int k = 0; k < 3; k++) x[k] = x[k] / n;
 }
@@ -83,7 +83,7 @@ __device__ __forceinline__ void face_light(const S N[3], const S pos[3], const L
         const S hv = 1.0f - dmax(dot3(H, V), 0.f);
         const S hv2 = hv * hv;
         const S p5 = (hv2 * hv2) * hv;                          // pow(1 - cosTheta, 5)
-        S den4 = dmax((NdotV * 4.0f) * NdotL, 0.01f);          // clamp(4 N.V N.L, 0.01) :125-128
+        S den4 = dclamp_min((NdotV * 4.0f) * NdotL, 0.01f);    // clamp(4 N.V N.L, min=0.01) :125-128
         const R ndf_g = NDF * G;
 #pragma unroll
         for (int c = 0; c < 3; c++) {
@@ -233,9 +233,10 @@ k_surface_lighting_bwd(const float* __restrict__ vertices, const int32_t* __rest
     // The normal's value and norm are the forward's float64 ones: on a sliver the float32 cross product and its norm
     // cancel, and the derivative would be taken at another normal (and the relu branches chosen there).  Only c's
     // partials come from the float32 duals; each is a sum of edge components, free of that cancellation.  They pass
-    // through normalize's Jacobian (I - N N^T) / |c|, or I / 1e-12 on its eps path, where the norm is the constant.
+    // through normalize's Jacobian (I - N N^T) / |c|, or I / 1e-12 on its eps path, where the norm is the constant
+    // (clamp_min's rule: |c| == 1e-12 exactly still differentiates through the norm).
     const float n = (float)fmax(len, 1e-12), inv = 1.f / n;
-    const bool on_eps = !(len > 1e-12);
+    const bool on_eps = !(len >= 1e-12);
     D Nd[3];
 #pragma unroll
     for (int j = 0; j < 3; j++) Nd[j].v = N[j];

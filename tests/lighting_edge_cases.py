@@ -187,12 +187,12 @@ def nm_clamp_bounds(B=2, T=33, seed=2):
     return sc
 
 
-def head(seed=0):
+def head(seed=0, faces=66282):
     """The demo 1.5 head's size on the normal-map path: B = 1, 66 282 faces, T = 225 (tools/time_normal_lighting.py's
-    synthetic mesh with finite TBNs)."""
+    synthetic mesh with finite TBNs); `faces` keeps the first that many."""
     rng = np.random.default_rng(seed)
     v, f = wl.uv_sphere(194, 172, jitter=0.002)
-    f = f[:66282].astype(np.int32)
+    f = f[:faces].astype(np.int32)
     nf, T = f.shape[0], 225
     tbn = jio.create_TBN(rng.uniform(0, 1, (nf, 3, 2)).astype(F32), v[f])
     tbn = np.where(np.isfinite(tbn), tbn, 0).astype(F32)[None]
@@ -296,3 +296,143 @@ def run(sc, dev, dtype, fused, grads=True):
     out.backward(torch.from_numpy(sc["gout"]).to(dev, dtype))
     g = {k: (None if t.grad is None else t.grad.cpu().double().numpy()) for k, t in ts.items()}
     return out.detach().cpu().double().numpy(), g
+
+
+def kernel_args(sc, backward=True, grads=None):
+    """The arguments Lighting hands the fused kernel for scene sc, as oracle.lighting.args_from_call returns them, built
+    on the host (no GPU): faces repeated over the vertex batch, the eye rows, per-face materials broadcast over the
+    texels on the normal-map path, the light direction normalised in float32.  grads: the gradients requested (all of
+    the path's by default)."""
+    import torch
+    import torch.nn.functional as F
+    nm = "nt" in sc
+    B, nf = sc["tex"].shape[:2]
+    T = sc["tex"][0, 0].size // 3
+    L = sc["light"]
+    spec = sc["eye"] is not None
+    d = F.normalize(torch.tensor([float(x) for x in L["directions"]], dtype=torch.float32), dim=0, eps=1e-12).numpy()
+    a = dict(vertices=sc["v"].astype(F32), faces=np.repeat(sc["f"][None], sc["v"].shape[0], 0).astype(np.int32),
+             textures=sc["tex"].astype(F32), eye=None if not spec else sc["eye"].astype(F32),
+             light=dict(amb_i=F32(L["intensity_ambient"]), amb_c=np.asarray(L["color_ambient"], F32),
+                        dir_i=F32(L["intensity_directionals"]), dir_c=np.asarray(L["color_directionals"], F32),
+                        dir=d.astype(F32), with_specular=spec))
+    a.update(B=B, Bv=sc["v"].shape[0], Bf=sc["v"].shape[0], Be=0 if not spec else sc["eye"].shape[0], nv=sc["v"].shape[1],
+             nf=nf, T=T)
+    if nm:
+        met = np.broadcast_to(sc["met"], (B, nf, T, 1)).astype(F32) if spec else None
+        rou = np.broadcast_to(sc["rou"], (B, nf, T, 1)).astype(F32) if spec else None
+        a.update(normal_textures=sc["nt"].astype(F32), tbn=sc["tbn"].astype(F32), metallic=met, roughness=rou,
+                 Bn=sc["nt"].shape[0], n_nf=nf, n_T=T, Bt=sc["tbn"].shape[0], t_nf=nf)
+    else:
+        a.update(metallic=sc["met"].astype(F32) if spec else None, roughness=sc["rou"].astype(F32) if spec else None,
+                 Tm=sc["met"][0, 0].size if spec else 0)
+    if backward:
+        grads = (NM_GRADS if nm else FLAT_GRADS) if grads is None else grads
+        a["grad_out"] = sc["gout"].astype(F32)
+        for k in grads:
+            src = dict(vertices=a["vertices"], textures=a["textures"], normal_textures=a.get("normal_textures"),
+                       metallic=a["metallic"], roughness=a["roughness"])[k]
+            a["grad_" + k] = None if src is None else np.empty_like(src)
+    return a
+
+
+# ---- equality at the clamp_min kinks ----------------------------------------------------------------------------------
+
+EPS12 = F32(1e-12)
+# a face whose centroid is exactly 0 (v, w, -v - w, dyadic): the forward's ((v0 + v1) + v2) / 3 and the flat backward's
+# ((v0 + v1) + v2) * (1 / 3) agree on it, so both evaluations see the same V; its normal is (1, 1, 0.5) / 1.5
+ZERO_FACE = F32([[0.25, -0.25, 0.0], [0.0, 0.125, -0.25], [-0.25, 0.125, 0.25]])
+
+
+def eps_texel():
+    """A float32 (x, y, 0) near 1e-12 (0.6, 0.8, 0) whose norm as the kernels form it, sqrt((x x + y y) + 0 0), is
+    exactly 1e-12f.  Through an identity TBN it is the texel normal itself (products by 1 and 0 are exact); a unit axis
+    would be unlit (x, z) or parallel to the axis light (y), where N.L's derivative vanishes."""
+    x = (F32(0.6e-12) + np.arange(-300, 300) * np.spacing(F32(0.6e-12))).astype(F32)
+    y = np.sqrt(np.float64(EPS12) ** 2 - np.float64(x) ** 2).astype(F32)
+    n = np.sqrt((x * x + y * y) + F32(0) * F32(0))
+    hit = np.flatnonzero(n == EPS12)
+    assert hit.size, "no texel normal of norm 1e-12f"
+    return F32([x[hit[0]], y[hit[0]], 0])
+
+
+def _den4_eye(N, L):
+    """An eye over the zero-centroid face for which the kernels' float32 den4 = (N.V * 4) * N.L is exactly 0.01f, with
+    N the normal as the kernel forms it: found among small float32 nudges of a grazing eye, with the emulation's own
+    normalize3 and dot3."""
+    from oracle import lighting as OL
+    from oracle.numbers import Walk
+    N64 = np.float64(N)
+    NdotL = float(N64 @ np.float64(L))
+    u = np.cross(N64, [0.0, 0.0, 1.0])
+    u /= np.linalg.norm(u)
+    want = 0.01 / (4 * NdotL)                      # N.V
+    base = 2.0 * (np.sqrt(1 - want ** 2) * u + want * N64)
+    k = np.arange(-600, 600)
+    w2 = np.cross(N64, u)
+    eyes = (base[None, None] + 1e-7 * (k[:, None, None] * N64 + k[None, :, None] * w2)).reshape(-1, 3).astype(F32)
+    w = Walk()
+    V = OL.normalize3(w, [eyes[:, j] - F32(0) for j in range(3)], F32(1e-12))
+    Nc = [np.full(len(eyes), F32(N[j])) for j in range(3)]
+    NdotV = np.maximum(OL.dot3(Nc, V), F32(0))
+    NdL = np.maximum(OL.dot3(Nc, [F32(x) for x in L]), F32(0))
+    den4 = (NdotV * F32(4)) * NdL
+    hit = np.flatnonzero(den4 == F32(0.01))
+    assert hit.size, "no eye puts den4 on 0.01f"
+    return eyes[hit[0]]
+
+
+def equality(nm, spec, B=4, T=4, seed=7):
+    """One mesh (Bv = 1) for four eyes, with a face whose centroid is exactly 0 (key `face`) under the axis light:
+        eye 0 = (1e-12f, 0, 0):   V = eye - pos has norm exactly 1e-12f, normalize's eps (sqrt(fl(x^2)) == x);
+        eye 1 = (1e-12f, -1, 0):  V = (1e-12f, -1, 0), V + L = (1e-12f, 0, 0): H's norm exactly 1e-12f;
+        eye 2: den4 = (N.V * 4) * N.L exactly 0.01f (found by _den4_eye);
+        eye 3: an ordinary eye.
+    On the normal-map path that face's TBN is the identity, texel 0's tangent-space normal n_t is EPS_TEXEL (norm
+    exactly 1e-12f, lit: N.L = 0.8) and its other texels carry the face normal.  spec=False drops the eyes (diffuse branch only)."""
+    from oracle import lighting as OL
+    rng = np.random.default_rng(seed)
+    vb, f = sphere(1, seed)
+    vb, f, idx = append(vb, f, ZERO_FACE[None])
+    fz = int(idx[0])
+    nf = f.shape[0]
+    L = F32([0, 1, 0])
+    if nm:
+        tbn = _tbn(rng, vb, f)[None].astype(F32)
+        tbn[0, fz] = np.eye(3, dtype=F32)
+        nt = _tangent_normals(rng, (1, nf, T))
+        Nf = flat_normals(vb, f)[0, fz].astype(F32)
+        nt[0, fz] = Nf
+        nt[0, fz, 0] = eps_texel()
+        from oracle.numbers import Walk
+        N = [x[0] for x in OL._texel_normal(Walk(), F32, [np.atleast_1d(Nf[j]) for j in range(3)],
+                                            [np.atleast_1d(F32(x)) for x in np.eye(3, dtype=F32).reshape(-1)])]
+    else:
+        N, _, _, _ = OL._normal_f64(vb[0][f[fz]].reshape(1, 9).astype(F32), None, F32)
+        N = [x[0] for x in N]
+    eye = F32([[EPS12, 0, 0], [EPS12, -1, 0], [0, 0, 0], [0.4, 2.2, 1.6]])
+    eye[2] = _den4_eye(N, L)
+    tex = rng.uniform(0.05, 0.9, (B, nf, T, 3)).astype(F32)
+    met, rou = _materials(rng, B, nf, (T,))
+    sc = dict(v=vb, f=f, tex=tex, met=met, rou=rou, eye=eye if spec else None,
+              gout=rng.uniform(-1, 1, tex.shape).astype(F32), light=AXIS_LIGHT, face=fz)
+    if nm:
+        sc.update(nt=nt, tbn=tbn)
+    return sc
+
+
+def shared_vertex(n=1000, B=4, nm=False, T=9, seed=8):
+    """A fan of n faces around one apex (vertex 0), one mesh (Bv = 1) for B eyes: the apex's grad_vertices entries sum
+    3 B n float atomics (the normal-map path: B n), so term_sums' bound carries large n."""
+    rng = np.random.default_rng(seed)
+    ang = np.linspace(0, 2 * np.pi, n, endpoint=False)
+    ring = np.stack([np.cos(ang), 0.3 + 0.05 * np.sin(7 * ang), np.sin(ang)], 1)
+    v = np.concatenate([[[0.0, 1.0, 0.0]], ring]).astype(F32)[None]
+    f = np.stack([np.zeros(n), 1 + (np.arange(n) + 1) % n, 1 + np.arange(n)], 1).astype(np.int32)
+    tex = rng.uniform(0, 1.3, (B, n, T, 3)).astype(F32)
+    met, rou = _materials(rng, B, n, (T,))
+    sc = dict(v=v, f=f, tex=tex, met=met, rou=rou, eye=EYES4[:B], gout=rng.uniform(-1, 1, tex.shape).astype(F32),
+              light=LIGHT)
+    if nm:
+        sc.update(nt=_tangent_normals(rng, (1, n, T)), tbn=_tbn(rng, v, f)[None].astype(F32))
+    return sc

@@ -2,7 +2,7 @@
 oracle/mesh_loss.py) against float64 references on the cases of geometry_edge_cases.py, and the host-built tables of
 LaplacianLoss / FlattenLoss against the reference's dense matrix and edge scan.  No GPU.
 
-Per-entry bound.  Each emulated term is re-evaluated with `EV` numbers: a float64 value plus a running bound on how far
+Per-entry bound.  Each emulated term is re-evaluated with `EV` numbers (oracle/numbers.py): a float64 value plus a running bound on how far
 the float32 evaluation of the same expression can be from the exact one (every operation: propagated input error plus
 one rounding u = 2^-24 of the result, 2^-52 for the float64 value's own rounding and 2^-149 for gradual underflow).  The
 sum of those per-term bounds is the bound on |exact sum of the emulated terms - float64 reference| for that entry.
@@ -15,74 +15,9 @@ import torch
 import jrender_b200 as jr
 from oracle import mesh_loss as oml
 from oracle import preraster as opr
+from oracle.numbers import EV
+from oracle.numbers import check_terms as _check_terms
 from tests import geometry_edge_cases as gec
-
-U = 2.0 ** -24
-U64 = 2.0 ** -52
-TINY = 2.0 ** -149
-
-
-class EV:
-    """float64 value `v` and a bound `e` on |float32 evaluation - exact value| of the expression that produced it."""
-
-    def __init__(self, v, e=None):
-        self.v = np.asarray(v, np.float64)
-        self.e = np.zeros_like(self.v) if e is None else np.asarray(e, np.float64)
-
-    @staticmethod
-    def of(x):
-        return x if isinstance(x, EV) else EV(x)
-
-    @staticmethod
-    def _round(v, prop):
-        return EV(v, prop + (U + U64) * (np.abs(v) + prop) + TINY)
-
-    def __getitem__(self, i):
-        return EV(self.v[i], self.e[i])
-
-    def __setitem__(self, i, x):
-        x = EV.of(x)
-        self.v[i], self.e[i] = x.v, x.e
-
-    def __neg__(self):
-        return EV(-self.v, self.e)
-
-    def __add__(self, o):
-        o = EV.of(o)
-        return EV._round(self.v + o.v, self.e + o.e)
-
-    __radd__ = __add__
-
-    def __sub__(self, o):
-        o = EV.of(o)
-        return EV._round(self.v - o.v, self.e + o.e)
-
-    def __rsub__(self, o):
-        return EV.of(o) - self
-
-    def __mul__(self, o):
-        o = EV.of(o)
-        return EV._round(self.v * o.v, np.abs(self.v) * o.e + np.abs(o.v) * self.e + self.e * o.e)
-
-    __rmul__ = __mul__
-
-    def __truediv__(self, o):
-        o = EV.of(o)
-        with np.errstate(all="ignore"):
-            q = self.v / o.v
-            den = np.abs(o.v) - o.e
-            prop = np.where(den > 0, (self.e + np.abs(q) * o.e) / den, np.inf)
-        return EV._round(q, prop)
-
-    def __rtruediv__(self, o):
-        return EV.of(o) / self
-
-    def sqrt(self):
-        with np.errstate(all="ignore"):
-            r = np.sqrt(np.maximum(self.v, 0))
-            prop = np.minimum(np.where(r > 0, self.e / r, np.inf), np.sqrt(self.e))
-        return EV._round(r, prop)
-
 
 def _ev_sums(slots, terms, size):
     """Per entry: float64 sum of the EV values and sum of their error bounds."""
@@ -90,16 +25,6 @@ def _ev_sums(slots, terms, size):
     np.add.at(s, slots, terms.v.reshape(-1))
     np.add.at(e, slots, terms.e.reshape(-1))
     return s, e
-
-
-def _check_terms(f32, ev):
-    """Every emulated float32 term is within its EV bound of the float64 value of the same expression (where that bound
-    is finite), and NaN wherever that value is NaN."""
-    f32 = np.asarray(f32, np.float64)
-    ok = np.isfinite(ev.v) & np.isfinite(ev.e)
-    assert np.isfinite(f32[ok]).all()
-    assert np.all(np.abs(f32 - ev.v)[ok] <= ev.e[ok])
-    assert np.isnan(f32[np.isnan(ev.v)]).all()
 
 
 # ---------------------------------------------------------------- projection

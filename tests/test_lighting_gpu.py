@@ -5,6 +5,8 @@ tests/golden/ref_host_lighting_stage.npz) and against the op-by-op PyTorch mirro
 normals / view vector, textures through the clamp) against the mirror's autograd in float64.
 Stated tolerances: lit textures 2e-5 of max (the golden's own tolerance on CPU; GGX ratios amplify ulps), gradients
 1e-4 of max |grad| (float32 forward-mode derivatives vs float64 reverse mode).
+Every fused call is also held to the kernels' float32 emulation (test_lighting_edges_gpu.hold_to_emulation): lit
+textures and per-texel gradients bit for bit, vertex gradients within the float atomics' order bound.
 """
 import os
 
@@ -14,6 +16,8 @@ import torch
 
 import jrender_b200 as jr
 from jrender_b200 import workloads as wl
+
+from tests.test_lighting_edges_gpu import hold_to_emulation, kernel_calls  # noqa: F401 (fixture)
 
 pytestmark = pytest.mark.gpu
 G = os.path.join(os.path.dirname(__file__), "golden")
@@ -29,7 +33,7 @@ def _mesh(g, dev, spec, dtype=torch.float32):
 
 
 @pytest.mark.parametrize("spec", [True, False])
-def test_fused_lighting_matches_reference_python_golden(cuda_device, spec):
+def test_fused_lighting_matches_reference_python_golden(cuda_device, kernel_calls, spec):
     g = np.load(os.path.join(G, "ref_host_lighting_stage.npz"))
     eyes = torch.from_numpy(g["eyes"]).to(cuda_device)
     light = jr.Lighting()
@@ -41,10 +45,11 @@ def test_fused_lighting_matches_reference_python_golden(cuda_device, spec):
     mirror.fused = False
     out2 = mirror(_mesh(g, cuda_device, spec), eyes).textures.cpu().numpy()
     assert np.abs(out - out2).max() <= 2e-5 * np.abs(ref).max()
+    hold_to_emulation(kernel_calls)
 
 
 @pytest.mark.parametrize("spec,tex6", [(True, False), (False, False), (True, True)])
-def test_fused_lighting_gradients_match_float64_autograd(cuda_device, spec, tex6):
+def test_fused_lighting_gradients_match_float64_autograd(cuda_device, kernel_calls, spec, tex6):
     rng = np.random.default_rng(5)
     v, f = wl.sphere_by_faces(280)
     B = 3
@@ -74,6 +79,7 @@ def test_fused_lighting_gradients_match_float64_autograd(cuda_device, spec, tex6
     assert np.abs(b[1]).max() > 0
     assert np.abs(a[1] - b[1]).max() <= 1e-4 * np.abs(b[1]).max(), np.abs(a[1] - b[1]).max() / np.abs(b[1]).max()
     assert np.abs(a[2] - b[2]).max() <= 1e-4 * np.abs(b[2]).max()
+    hold_to_emulation(kernel_calls)
 
 
 def test_renderer_uses_the_fused_lighting_and_counts_one_launch(cuda_device):

@@ -8,6 +8,8 @@ Tolerances:
   in a different order each run, and the two lighting paths' lit textures differ in the last bits.  Measured on an
   NVIDIA H100 80GB HBM3 (700 W): 2.1e-6 (metallic) and 5.9e-6 (roughness) fused vs op-by-op, against a fused run-to-run
   spread of 4e-8;
+- every fused call also against the kernels' float32 emulation (test_lighting_edges_gpu.hold_to_emulation): lit
+  textures and per-texel gradients bit for bit, vertex gradients within the float atomics' order bound;
 - demo convergence: the final loss is at most CONVERGED of the first.  Measured on the same card: 0.0052 (demo 5,
   20 iterations) and 0.0006 (demo 6, 15 iterations); the thresholds leave a margin of about 6x and 15x.
 """
@@ -20,6 +22,8 @@ import torch
 import jrender_b200 as jr
 from jrender_b200 import _lib
 from jrender_b200 import workloads as wl
+
+from tests.test_lighting_edges_gpu import hold_to_emulation, kernel_calls  # noqa: F401 (fixture)
 
 pytestmark = pytest.mark.gpu
 G = os.path.join(os.path.dirname(__file__), "golden")
@@ -89,7 +93,7 @@ def _lit_grads(dev, scene, eyes, dtype, fused, spec=True, material_grad=True):
 
 @pytest.mark.parametrize("eyes", sorted(EYES))
 @pytest.mark.parametrize("tex6", [False, True])
-def test_material_gradients_match_float64_autograd(cuda_device, tex6, eyes):
+def test_material_gradients_match_float64_autograd(cuda_device, kernel_calls, tex6, eyes):
     scene = _scene(tex6)
     out, got = _lit_grads(cuda_device, scene, EYES[eyes], torch.float32, True)
     out64, ref = _lit_grads(cuda_device, scene, EYES[eyes], torch.float64, False)
@@ -99,10 +103,11 @@ def test_material_gradients_match_float64_autograd(cuda_device, tex6, eyes):
         a, b = a.double().cpu().numpy(), b.cpu().numpy()
         assert np.abs(b).max() > 0, name
         assert np.abs(a - b).max() <= 1e-4 * np.abs(b).max(), (name, np.abs(a - b).max() / np.abs(b).max())
+    hold_to_emulation(kernel_calls)
 
 
 @pytest.mark.parametrize("tex6", [False, True])
-def test_material_gradients_without_specular(cuda_device, tex6):
+def test_material_gradients_without_specular(cuda_device, kernel_calls, tex6):
     """with_specular off: neither path connects the materials to the output (no gradient), the other gradients still
     match; at the C ABI the kernel writes exact zeros into requested material gradients."""
     scene = _scene(tex6)
@@ -129,10 +134,11 @@ def test_material_gradients_without_specular(cuda_device, tex6):
                   _lib._f3([0.3, 1, -0.4]), with_spec)
         torch.cuda.synchronize()
         assert bool((gm == 0).all()) and bool((gr == 0).all()), (with_spec, e is None)
+    hold_to_emulation(kernel_calls)
 
 
 @pytest.mark.parametrize("tex6", [False, True])
-def test_material_gradients_leave_the_other_gradients_unchanged(cuda_device, tex6):
+def test_material_gradients_leave_the_other_gradients_unchanged(cuda_device, kernel_calls, tex6):
     """Requesting material gradients changes neither the lit textures nor the texture gradients (bit for bit) nor the
     vertex gradients (beyond the float atomics' summation order)."""
     scene = _scene(tex6)
@@ -141,6 +147,7 @@ def test_material_gradients_leave_the_other_gradients_unchanged(cuda_device, tex
     assert torch.equal(out_a, out_b) and torch.equal(a[1], b[1])
     assert float((a[0] - b[0]).abs().max()) <= 1e-6 * float(b[0].abs().max())
     assert b[2] is None and b[3] is None
+    hold_to_emulation(kernel_calls)
 
 
 def test_material_gradients_take_the_fused_path(cuda_device):

@@ -6,6 +6,8 @@ Tolerances:
 - normal textures baked on the GPU vs the golden's oracle bake: 1e-5 (the bake itself is held to 2e-6, the
   normalize(n * 2 - 1) that follows scales that by at most 2 / |2n - 1|);
 - fused float32 gradients vs the mirror's float64 autograd: 1e-4 of max |grad|, as tests/test_lighting_gpu.py states;
+- every fused call also against the kernels' float32 emulation (test_lighting_edges_gpu.hold_to_emulation): lit
+  textures and per-texel gradients bit for bit, vertex gradients within the float atomics' order bound;
 - the normal-map fit: the final loss is at most FIT_FRACTION of the first.  Measured on an NVIDIA H100 80GB HBM3
   (700 W): 0.056 after 40 iterations on the generated sphere; the threshold leaves a margin of about 3.5x.
 """
@@ -19,6 +21,8 @@ import jrender_b200 as jr
 from jrender_b200 import _lib
 from jrender_b200 import io as jio
 from jrender_b200 import workloads as wl
+
+from tests.test_lighting_edges_gpu import hold_to_emulation, kernel_calls  # noqa: F401 (fixture)
 
 pytestmark = pytest.mark.gpu
 G = os.path.join(os.path.dirname(__file__), "golden")
@@ -70,7 +74,7 @@ def _golden_mesh(g, dev, spec, dtype=torch.float32):
 
 
 @pytest.mark.parametrize("tag,spec", [("specular", True), ("diffuse", False)])
-def test_fused_forward_matches_golden_and_mirror(cuda_device, g, tag, spec):
+def test_fused_forward_matches_golden_and_mirror(cuda_device, kernel_calls, g, tag, spec):
     eyes = torch.from_numpy(g["lit_eyes"]).to(cuda_device)
     light = jr.Lighting(**LIGHT)
     m = _golden_mesh(g, cuda_device, spec)
@@ -85,6 +89,7 @@ def test_fused_forward_matches_golden_and_mirror(cuda_device, g, tag, spec):
         x = x.cpu().numpy()
         assert np.abs(x - ref).max() <= 2e-5 * np.abs(ref).max()
     assert float((fused - mirror).abs().max()) <= 2e-5
+    hold_to_emulation(kernel_calls)
 
 
 EYES = {"per_batch": [[0.0, 0.3, -2.7], [1.0, 1.5, -2.0], [-2.0, 0.3, 1.0]],
@@ -144,7 +149,7 @@ def _compare(got, ref, need=NAMES):
 
 @pytest.mark.parametrize("nb", [1, 3])
 @pytest.mark.parametrize("eyes", sorted(EYES))
-def test_gradients_match_float64_autograd(cuda_device, eyes, nb):
+def test_gradients_match_float64_autograd(cuda_device, kernel_calls, eyes, nb):
     sc = _scene(nb)
     out, got = _grads(cuda_device, sc, EYES[eyes], torch.float32, True)
     out64, ref = _grads(cuda_device, sc, EYES[eyes], torch.float64, False)
@@ -152,10 +157,11 @@ def test_gradients_match_float64_autograd(cuda_device, eyes, nb):
     assert bool((out64 >= 1).any())   # texels that saturate the clamp are in the scene
     _compare(got, ref)
     assert float(got[2][:, 7, 4].abs().max()) == 0.0   # the zero normal: every relu is at its kink
+    hold_to_emulation(kernel_calls)
 
 
 @pytest.mark.parametrize("nb", [1, 3])
-def test_gradients_without_specular(cuda_device, nb):
+def test_gradients_without_specular(cuda_device, kernel_calls, nb):
     """Without the Cook-Torrance branch the vertices reach nothing: autograd has no path to them, the kernel writes 0."""
     sc = _scene(nb)
     need = NAMES[:3]
@@ -163,11 +169,12 @@ def test_gradients_without_specular(cuda_device, nb):
     _, ref = _grads(cuda_device, sc, EYES["per_batch"], torch.float64, False, spec=False, need=need)
     assert ref[0] is None and float(got[0].abs().max()) == 0.0
     _compare([None] + got[1:], [None] + ref[1:], need[1:])
+    hold_to_emulation(kernel_calls)
 
 
 @pytest.mark.parametrize("need", [("textures",), ("normal_textures",), ("vertices",), ("metallic", "roughness"),
                                   ("vertices", "normal_textures")])
-def test_gradient_subsets(cuda_device, need):
+def test_gradient_subsets(cuda_device, kernel_calls, need):
     """Each gradient is written only when requested, and requesting fewer changes none of the others: per-texel ones bit
     for bit, the vertex gradient beyond the float atomics' order."""
     sc = _scene(1)
@@ -183,6 +190,7 @@ def test_gradient_subsets(cuda_device, need):
             assert torch.equal(a, b), name
     _, ref = _grads(cuda_device, sc, EYES["per_batch"], torch.float64, False, need=need)
     _compare(got, ref, need)
+    hold_to_emulation(kernel_calls)
 
 
 def test_grad_requiring_eye_or_tbn_runs_op_by_op(cuda_device):
