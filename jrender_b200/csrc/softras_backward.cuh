@@ -3,11 +3,18 @@
 //
 // The reference issues 9 + 3T scalar global atomicAdd per (pixel, face) pair.  Here every lane walks its own <=K saved
 // ids, reads the face record straight from the L1-resident record array, and adds its 12 gradient values (9 vertex +
-// 3 colour for T == 1) with THREE 16-byte REDG.E.ADD.F32x4 into a padded accumulator [B*nf][12];
+// 3 colour for T == 1) with at most THREE 16-byte REDG.E.ADD.F32x4 into a padded accumulator [B*nf][12];
 // k_softras_bwd_finalize then unpacks it into grad_face_vertices [.,9] and grad_textures [.,1,3] (36-byte rows cannot
 // take 16-byte atomics directly).  Atomic packets drop 4x against the reference and no zero-fill of the outputs is
 // needed.  Before the atomics of a step, lanes ^1 and ^8 (horizontal / vertical neighbour pixels) that hold the same
 // face add their values by shuffle into the lower lane (merge_same_face).
+//
+// A packet whose four values are all +-0 is not issued (add_nonzero).  The accumulator rows are laid out by what
+// vanishes together, so that more packets are all zero: [v0.x v0.y v1.x v1.y] [v2.x v2.y v0.z v1.z] [v2.z t0 t1 t2].
+// The x/y terms carry D (1 - D), exactly 0 deep inside a face; the z and colour terms carry zp_softmax, which
+// underflows for faces far behind the front ones, and the z term of vertex k the clipped barycentric w_k, 0 outside the
+// triangle.  Counted on the oracle's terms (tools/count_softras_bwd_packets.py, DESIGN.md section 8), this issues 22 %
+// fewer packets than the interleaved layout issued unconditionally at C3, 27 % fewer for C5's silhouettes.
 //
 // Measured and dropped, all slower at C3: a walk in ascending face id (ids staged and sorted in shared memory so that
 // neighbouring lanes sit on the same record at the same step -- the sort costs more than the L1 sectors it saves);
@@ -214,6 +221,15 @@ __device__ __forceinline__ void merge_same_face(int& key, float gv[9], float gt[
     if (same && !lower) key = -1;
 }
 
+// Adds v to *a unless all of v is +-0.  The accumulators start at +0 and adding a zero leaves a sum unchanged, so
+// skipping changes no value.  The test runs on the merged sums: two subnormal terms can add up to a normal number.
+__device__ __forceinline__ void add_nonzero(float4* a, float4 v) {
+    if ((__float_as_uint(v.x) | __float_as_uint(v.y) | __float_as_uint(v.z) | __float_as_uint(v.w)) << 1) atomicAdd(a, v);
+}
+__device__ __forceinline__ void add_nonzero(float* a, float v) {
+    if (__float_as_uint(v) << 1) atomicAdd(a, v);
+}
+
 // ---------------------------------------------------------------- per-lane walk + vector atomics
 template <int DIST, int RGB, bool EXACT>
 __global__ void __launch_bounds__(B200R_TILE_THREADS, kBwdMinBlocks)
@@ -292,18 +308,18 @@ k_softras_backward_lane(const SoftRasParams P, const FaceRec* __restrict__ recs,
         }
         if (key >= 0) {
             float4* a = reinterpret_cast<float4*>(bacc + (size_t)key * 12);
-            atomicAdd(a + 0, make_float4(gv[0], gv[1], gv[2], gv[3]));
-            atomicAdd(a + 1, make_float4(gv[4], gv[5], gv[6], gv[7]));
+            add_nonzero(a + 0, make_float4(gv[0], gv[1], gv[3], gv[4]));
+            add_nonzero(a + 1, make_float4(gv[6], gv[7], gv[2], gv[5]));   // silhouettes: gv[2], gv[5] are 0
             if (RGB != 2)   // silhouettes: gv[8] (a z gradient) and the colour gradients are identically 0
-                atomicAdd(a + 2, make_float4(gv[8], tex_in_acc ? gt[0] : 0.f, tex_in_acc ? gt[1] : 0.f, tex_in_acc ? gt[2] : 0.f));
+                add_nonzero(a + 2, make_float4(gv[8], tex_in_acc ? gt[0] : 0.f, tex_in_acc ? gt[1] : 0.f, tex_in_acc ? gt[2] : 0.f));
         }
         if (RGB != 2 && !tex_in_acc && fn >= 0) {
             if (P.tex_type == 0) {
 #pragma unroll
-                for (int k = 0; k < 3; k++) atomicAdd(bgt + ((size_t)fn * T + texel) * 3 + k, gt[k]);
+                for (int k = 0; k < 3; k++) add_nonzero(bgt + ((size_t)fn * T + texel) * 3 + k, gt[k]);
             } else {
 #pragma unroll
-                for (int c = 0; c < 9; c++) atomicAdd(bgt + (size_t)fn * 9 + c, gt[c]);
+                for (int c = 0; c < 9; c++) add_nonzero(bgt + (size_t)fn * 9 + c, gt[c]);
             }
         }
         fn = fn_next;
@@ -311,8 +327,8 @@ k_softras_backward_lane(const SoftRasParams P, const FaceRec* __restrict__ recs,
     }
 }
 
-// Unpacks the padded accumulator: grad_face_vertices[i][0..8] and, for T == 1 surface textures,
-// grad_textures[i][0..2].
+// Unpacks the padded accumulator [v0.x v0.y v1.x v1.y] [v2.x v2.y v0.z v1.z] [v2.z t0 t1 t2]:
+// grad_face_vertices[i][0..8] and, for T == 1 surface textures, grad_textures[i][0..2].
 __global__ void __launch_bounds__(256)
 k_softras_bwd_finalize(const float* __restrict__ gacc, float* __restrict__ grad_faces, float* __restrict__ grad_textures,
                        int total_faces, int tex_in_acc) {
@@ -321,9 +337,9 @@ k_softras_bwd_finalize(const float* __restrict__ gacc, float* __restrict__ grad_
     const float4* a = reinterpret_cast<const float4*>(gacc + (size_t)i * 12);
     const float4 v0 = a[0], v1 = a[1], v2 = a[2];
     float* g = grad_faces + (size_t)i * 9;
-    g[0] = v0.x; g[1] = v0.y; g[2] = v0.z; g[3] = v0.w;
-    g[4] = v1.x; g[5] = v1.y; g[6] = v1.z; g[7] = v1.w;
-    g[8] = v2.x;
+    g[0] = v0.x; g[1] = v0.y; g[2] = v1.z;
+    g[3] = v0.z; g[4] = v0.w; g[5] = v1.w;
+    g[6] = v1.x; g[7] = v1.y; g[8] = v2.x;
     if (tex_in_acc) {
         float* t = grad_textures + (size_t)i * 3;
         t[0] = v2.y; t[1] = v2.z; t[2] = v2.w;
