@@ -122,7 +122,9 @@ k_bake_textures_n3mr(const float* __restrict__ image, const float* __restrict__ 
         float v = __ldg(faces_uv + (size_t)fn * 6 + k);
         if (WRAP == 0) v = ref_mod(v, 1.f);                                            // REPEAT :151-156
         else if (WRAP == 1) v = ref_mod(v, 2.f) < 1.f ? ref_mod(v, 1.f) : 1.f - ref_mod(v, 1.f);   // MIRRORED_REPEAT :157-167
-        else if (WRAP == 2) v = fmaxf(fminf(v, 1.f), 0.f);                             // CLAMP_TO_EDGE :168-173
+        // CLAMP_TO_EDGE :168-173.  fminf(NaN, 1) is 1; spelled out because nvcc lowers the clamp to a saturating add,
+        // which takes NaN to 0
+        else if (WRAP == 2) v = v != v ? 1.f : fmaxf(fminf(v, 1.f), 0.f);
         face[k] = v;
     }
     float* texture = textures + i * 3;

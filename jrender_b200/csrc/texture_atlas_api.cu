@@ -47,7 +47,9 @@ __device__ __forceinline__ void atlas_weights(const float* __restrict__ tri, int
 #pragma unroll
     for (int k = 0; k < 3; k++) {
         w[k] = face_inv[3 * k + 0] * (float)x + face_inv[3 * k + 1] * (float)y + face_inv[3 * k + 2];
-        w[k] = (float)fmax(fmin((double)w[k], 1.), 0.);
+        // fmin(NaN, 1.) is 1 (a degenerate tile divides by zero); spelled out because nvcc lowers the clamp to a
+        // saturate, which takes NaN to 0
+        w[k] = w[k] != w[k] ? 1.f : (float)fmax(fmin((double)w[k], 1.), 0.);
         w_sum += w[k];
     }
 #pragma unroll

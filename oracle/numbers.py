@@ -94,6 +94,23 @@ class EV:
         return EV._round(r, prop)
 
 
+def cuda_int(a):
+    """C float -> int conversion as the GPU does it (cvt.rzi.s32.f32 / .f64): truncation toward zero, saturating at
+    INT_MIN / INT_MAX, NaN -> 0.  Returned as int64 (numpy's own astype gives INT64_MIN for NaN and +-inf on x86)."""
+    a = np.nan_to_num(np.asarray(a, np.float64), nan=0.0, posinf=2147483647.0, neginf=-2147483648.0)
+    return np.clip(np.trunc(a), -2147483648.0, 2147483647.0).astype(np.int64)
+
+
+def fminf(a, b):
+    """CUDA fminf / fmin: the other operand where one is NaN (np.minimum would propagate the NaN)."""
+    return np.fmin(a, b)
+
+
+def fmaxf(a, b):
+    """CUDA fmaxf / fmax: the other operand where one is NaN."""
+    return np.fmax(a, b)
+
+
 def check_terms(f32, ev):
     """Every emulated float32 term is within its EV bound of the float64 value of the same expression (where that bound
     is finite), and NaN wherever that value is NaN."""

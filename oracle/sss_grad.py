@@ -32,6 +32,7 @@ Stretch and bake bounds are built the same way (stretch_bound(), bake()), with t
 import numpy as np
 import torch
 
+from . import bake as obake
 from . import sss as osss
 
 F32 = np.float32
@@ -297,25 +298,8 @@ def stretch_bound(world, passes, gu, gv):
 
 def bake_weights(faces_uv, R, H, W):
     """The SoftRas bake's per-texel flat indices [nf, T, 4] (clamped as the kernel clamps) and float32 bilinear
-    weights [nf, T, 4], in the kernel's promotions (oracle/bake.py)."""
-    T = R * R
-    wy, wx = np.divmod(np.arange(T), R)
-    lower = (wx + wy) < R
-    w0 = np.where(lower, (wx + 1. / 3.) / R, ((R - 1. - wx) + 2. / 3.) / R).astype(F32)
-    w1 = np.where(lower, (wy + 1. / 3.) / R, ((R - 1. - wy) + 2. / 3.) / R).astype(F32)
-    w2 = (1. - w0.astype(np.float64) - w1.astype(np.float64)).astype(F32)
-    f = np.asarray(faces_uv, F32)
-    pos_x = ((f[:, None, 0, 0] * w0 + f[:, None, 1, 0] * w1 + f[:, None, 2, 0] * w2) * F32(W - 1)).astype(F32)
-    pos_y = ((f[:, None, 0, 1] * w0 + f[:, None, 1, 1] * w1 + f[:, None, 2, 1] * w2) * F32(H - 1)).astype(F32)
-    ix, iy, iy1 = osss._f2i(pos_x), osss._f2i(pos_y), osss._f2i((pos_y + F32(1)).astype(F32))
-    wx1 = (pos_x - ix.astype(F32)).astype(F32)
-    wx0 = (F32(1) - wx1).astype(F32)
-    wy1 = (pos_y - iy.astype(F32)).astype(F32)
-    wy0 = (F32(1) - wy1).astype(F32)
-    i00, i10 = iy * W + ix, iy1 * W + ix
-    idx = np.clip(np.stack([i00, i10, i00 + 1, i10 + 1], -1), 0, H * W - 1)
-    wts = np.stack([wx0 * wy0, wx0 * wy1, wx1 * wy0, wx1 * wy1], -1).astype(F32)
-    return idx, wts
+    weights [nf, T, 4], in the kernel's promotions (oracle/bake.softras_taps)."""
+    return obake.softras_taps(faces_uv, R, H, W)
 
 
 def bake(image, faces_uv, R, is_update=None):
@@ -333,18 +317,19 @@ def bake(image, faces_uv, R, is_update=None):
 
 
 def bake_vjp(grad_textures, faces_uv, R, H, W, is_update=None, magnitude=False):
-    """The bake's adjoint [H, W, 3] (magnitude=True: of |g| w), and the count of contributions per pixel [H, W]."""
-    idx, wts = bake_weights(faces_uv, R, H, W)
-    g = grad_textures.double().abs() if magnitude else grad_textures.double()
-    if is_update is not None:
-        g = g * _t((np.asarray(is_update) != 0).astype(np.float64), g)[:, None, None]
+    """The bake's adjoint [H, W, 3] (magnitude=True: of |g| |w|; the weights extrapolate, and turn negative, for UVs
+    outside [0, 1]), and the count of contributions per pixel [H, W].  Faces with is_update == 0 take no part (their
+    weights may be non-finite)."""
+    keep = np.ones(grad_textures.shape[0], bool) if is_update is None else np.asarray(is_update) != 0
+    idx, wts = bake_weights(np.asarray(faces_uv, F32)[keep], R, H, W)
+    if magnitude:
+        wts = np.abs(wts)
+    g = grad_textures.double()[_t(keep, grad_textures)]
+    g = g.abs() if magnitude else g
     it, wt = _t(idx, g).reshape(-1), _t(wts.astype(np.float64), g)
     out = torch.zeros((H * W, 3), dtype=torch.float64, device=g.device)
     out.index_add_(0, it, (g[:, :, None, :] * wt[..., None]).reshape(-1, 3))
-    live = torch.ones(idx.shape, dtype=torch.float64, device=g.device)
-    if is_update is not None:
-        live = live * _t((np.asarray(is_update) != 0).astype(np.float64), g)[:, None, None]
-    n = torch.zeros(H * W, dtype=torch.float64, device=g.device).index_add_(0, it, live.reshape(-1))
+    n = torch.zeros(H * W, dtype=torch.float64, device=g.device).index_add_(0, it, torch.ones_like(it, dtype=torch.float64))
     return out.reshape(H, W, 3), n.reshape(H, W)
 
 

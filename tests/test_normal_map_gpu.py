@@ -3,8 +3,9 @@ the op-by-op mirror they replace.
 
 Tolerances:
 - lit textures, fused vs the golden and vs the mirror: 2e-5 of max, as for ref_host_lighting_stage;
-- normal textures baked on the GPU vs the golden's oracle bake: 1e-5 (the bake itself is held to 2e-6, the
-  normalize(n * 2 - 1) that follows scales that by at most 2 / |2n - 1|);
+- textures and normal textures baked on the GPU vs oracle/bake.py's emulation of the bake kernel on the same image:
+  bit for bit; vs the golden's (an older float64-weight oracle bake): 2e-6 and 1e-5 (the normalize(n * 2 - 1) that
+  follows scales the bake's difference by at most 2 / |2n - 1|);
 - fused float32 gradients vs the mirror's float64 autograd: 1e-4 of max |grad|, as tests/test_lighting_gpu.py states;
 - every fused call also against the kernels' float32 emulation (test_lighting_edges_gpu.hold_to_emulation): lit
   textures and per-texel gradients bit for bit, vertex gradients within the float atomics' order bound;
@@ -21,6 +22,7 @@ import jrender_b200 as jr
 from jrender_b200 import _lib
 from jrender_b200 import io as jio
 from jrender_b200 import workloads as wl
+from oracle import bake as obake
 
 from tests.test_lighting_edges_gpu import hold_to_emulation, kernel_calls  # noqa: F401 (fixture)
 
@@ -57,6 +59,13 @@ def test_loader_matches_reference(cuda_device, g, tmp_path, kind):
     assert np.abs(tex.numpy() - g["textures"]).max() <= 2e-6
     assert np.abs(nt.numpy() - g["normal_textures_" + kind]).max() <= 1e-5
     assert np.array_equal(tbn.numpy(), g["TBN"]) and np.array_equal(ftc.numpy(), g["face_texcoords"])
+    image = jio._imread_native01(os.path.join(str(tmp_path), MAPS[kind]))
+    image = jio.bump_to_normal_map(image) if image.ndim == 2 else image
+    nf = ftc.shape[0]
+    baked = obake.bake_textures_for_softras(np.ascontiguousarray(image[::-1]), ftc.numpy(), np.ones((nf, R * R, 3), np.float32),
+                                            np.ones(nf, np.int32))
+    want = jio._normalize_np(baked * 2 - 1, 2, 1e-12)
+    assert np.array_equal(nt.numpy().view(np.uint32), want.view(np.uint32))
     m = jr.Mesh.from_obj(path, load_texture=True, texture_res=R, normalization=True).to(cuda_device)
     assert tuple(m.normal_textures.shape) == (1,) + g["TBN"].shape[:1] + (R * R, 3)
     assert torch.equal(m.TBN.cpu(), torch.from_numpy(g["TBN"])[None])   # built before the normalization

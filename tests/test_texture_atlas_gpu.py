@@ -1,8 +1,9 @@
 """GPU tests of the texture-atlas export (csrc/texture_atlas_api.cu <- jrender/io/utils/create_texture_image.py; NMR
 volumes through the NMR sampler's trilinear fetch) and of the textured OBJ files it feeds.
 
-Tolerances: the SoftRas atlas is a texel copy, bit-equal to the numpy oracle (oracle/texture_atlas.py: same float32
-operations, no contraction on either side); the NMR atlas 2e-6 of the oracle (sums of eight products in [0, 1]).  Against
+Tolerances: both atlases are bit-equal to the numpy oracle (oracle/texture_atlas.py: same float32 operations in the
+same order, no contraction on either side), and the oracle chains (atlas -> 8-bit PNG -> bake, oracle/bake.py) are
+bit-equal to the product's save / load round trips.  Against
 the reference's own kernel (tests/golden/ref_atlas_gpu_*.npz) at most 1e-3 of the pixels may pick another texel: that
 build contracts a*b+c, which moves pixels on a cell boundary.  Round trips save_obj -> load_obj compare with the 8-bit
 PNG's value floor(255 clip(c)) / 255 to 1e-6.
@@ -55,7 +56,7 @@ def test_kernels_match_oracle(cuda_device, nf, R_out):
         for ts in (2, 3, 4):
             tex = rng.random((nf, ts, ts, ts, 3), dtype=np.float32)
             got = _atlas(t, tex, R_out, tw, H, W, cuda_device)
-            assert np.abs(got - oat.texture_atlas_n3mr(t, tex, R_out, tw, H, W)).max() <= 2e-6, (ts, "n3mr")
+            assert np.array_equal(got, oat.texture_atlas_n3mr(t, tex, R_out, tw, H, W)), (ts, "n3mr")
 
 
 def test_kernel_matches_reference_kernel_golden(cuda_device):
@@ -143,7 +144,7 @@ def _oracle_chain(textures, obj, R_out, kind):
 
 def test_spot_cow_round_trip(cuda_device, spot, tmp_path):
     """The textured cow: load (texture_res 4), Mesh.save_obj(save_texture=True), load again.  The reloaded texels equal
-    the oracle's chain to 2e-6; how far they moved from the loaded ones is printed (not asserted: the atlas holds one
+    the oracle's chain bit for bit; how far they moved from the loaded ones is printed (not asserted: the atlas holds one
     sample per pixel of a 16-pixel tile and 8 bits per channel)."""
     mesh = jr.Mesh.from_obj(spot, load_texture=True, texture_res=4).to(cuda_device)
     out = str(tmp_path / "cow.obj")
@@ -153,7 +154,7 @@ def test_spot_cow_round_trip(cuda_device, spot, tmp_path):
     orig = mesh.textures[0].cpu().numpy()
     got = back.textures[0].numpy()
     assert np.abs(back.vertices.numpy() - mesh.vertices.cpu().numpy()).max() <= 1e-7
-    assert np.abs(got - _oracle_chain(orig, out, 16, "softras")).max() <= 2e-6
+    assert np.array_equal(got, _oracle_chain(orig, out, 16, "softras"))
     d = np.abs(got - orig)
     print("\nspot cow round trip (texture_res 4, texture_res_out 16): |reloaded - original| mean %.5f max %.5f" % (d.mean(), d.max()))
 
@@ -167,7 +168,7 @@ def test_mesh_save_obj_nmr_and_vertex_colours(cuda_device, spot, tmp_path):
     mesh.save_obj(out, save_texture=True, texture_res_out=8)
     back = jr.Mesh.from_obj(out, load_texture=True, texture_res=4, dr_type='n3mr')
     assert tuple(back.textures.shape) == (1, 5856, 4, 4, 4, 3)
-    assert np.abs(back.textures[0].numpy() - _oracle_chain(mesh.textures[0].cpu().numpy(), out, 8, "n3mr")).max() <= 2e-6
+    assert np.array_equal(back.textures[0].numpy(), _oracle_chain(mesh.textures[0].cpu().numpy(), out, 8, "n3mr"))
     from jrender_b200 import workloads as wl
     v, f = wl.sphere_by_faces(280)
     col = torch.rand(1, v.shape[0], 3, device=cuda_device)
@@ -191,5 +192,5 @@ def test_demo4_save(cuda_device, spot, tmp_path):
     back = jr.Mesh.from_obj(out, load_texture=True, texture_res=4, dr_type='n3mr')
     assert tuple(back.textures.shape) == (1, 5856, 4, 4, 4, 3)
     fitted = torch.tanh(model.textures)[0].detach().cpu().numpy()
-    assert np.abs(back.textures[0].numpy() - _oracle_chain(fitted, out, 16, "n3mr")).max() <= 2e-6
+    assert np.array_equal(back.textures[0].numpy(), _oracle_chain(fitted, out, 16, "n3mr"))
     assert np.abs(back.vertices.numpy() - model.vertices[0].cpu().numpy()).max() <= 1e-7
