@@ -14,7 +14,8 @@
 //
 // Scheduling: a persistent grid pulls blocks from an atomic queue (head `tile_counter`) ordered by descending cost
 // (number of (pixel, face) pairs per block, computed by k_coarse_bin and bucket-sorted by k_tile_order): blocks at
-// poles / silhouettes of a mesh can cost 10x the mean and must start first.
+// poles / silhouettes of a mesh can cost 10x the mean and must start first.  Blocks no face rectangle touches (76 % at
+// C3) only store constants; they ride along with the shaded blocks (kFwdEmptyShare) rather than queueing behind them.
 #pragma once
 #include "softras_math.cuh"
 #include "softras_setup.cuh"
@@ -35,7 +36,7 @@ static_assert(B200R_BLOCK_W * B200R_BLOCK_H == kFwdLanes, "one lane per pixel of
 
 // resident one-warp CTAs per SM the register allocation must allow (96 registers).  H100, C3: forward 1.08 ms at 20, 1.10
 // at 16, 1.29 at 24 (16-record rounds, LDG staging); with bulk copies 1.017 at 20, 1.016 at 22, 1.017 at 18.  Spills
-// (ptxas, sm_90a): the C3 instantiation <2,1,false> 60 B stored / 64 B loaded at 96 registers; the others 0-44 B
+// (ptxas, sm_90a): the C3 instantiation <2,1,false> 60 B stored / 72 B loaded at 96 registers; the others 0-32 B
 constexpr int kFwdMinBlocks = 20;
 
 // ---- mbarrier / bulk-copy (TMA) helpers.  Records are staged by cp.async.bulk + mbarrier rather than LDG -> registers
@@ -324,13 +325,69 @@ __device__ __forceinline__ void finalize_pixel(const PixState& st, const SoftRas
     }
 }
 
+// per-pixel state before the first face, as :291-309 (background buffer is all zero, Q1); softmax_sum0 = exp(eps / gamma)
+template <int RGB>
+__device__ __forceinline__ PixState initial_state(const SoftRasParams& P, float softmax_sum0) {
+    PixState st;
+    st.softmax_sum = softmax_sum0;
+    st.softmax_max = P.eps;
+    if (RGB == 0) { st.sc0 = st.sc1 = st.sc2 = 0.f; }
+    else if (RGB == 1) { st.sc0 = st.sc1 = st.sc2 = 0.f * softmax_sum0; }
+    else { st.sc0 = st.sc1 = st.sc2 = 1.f; }
+    st.alpha = (P.alpha_func == 2) ? 1.f : 0.f;
+    st.depth_min = 10000000.f;
+    st.face_index_min = -1;
+    st.q_size = 0;
+    st.q_max_z = -1.f;
+    st.q_max_id = -1;
+    return st;
+}
+
+// Blocks no face rectangle touches: every pixel leaves with its initial state.  Lane j < ne holds queue entry j (ne <= 32,
+// warp-uniform).  Six constant planes and the terminator of the id lists, straight from registers, as 16-byte row
+// segments (is % 4 == 0 and K % 4 == 0): per block, lane l stores row (l >> 1) & 3, half l & 1 of colour plane l >> 3,
+// then lanes 0-15 the same of aggregate plane (l >> 3) & 1 and lanes 16-23 the id terminator -- two stores per lane.
+// The values and the lane's offsets are set up once per call, so a block costs its address and its stores.  Nothing
+// reads these stores back, so the warp does not wait for them.
+template <int RGB>
+__device__ __forceinline__ void store_empty_blocks(uint2 ee, int ne, const SoftRasParams& P, float softmax_sum0,
+                                                   float* __restrict__ soft_colors, float* __restrict__ aggrs_info,
+                                                   int* __restrict__ ids_out, int lane) {
+    const int is = P.is;
+    const size_t npix = (size_t)is * is;
+    float o[6];
+    finalize_pixel<RGB>(initial_state<RGB>(P, softmax_sum0), P, o[0], o[1], o[2], o[3], o[4], o[5]);
+    const int ch = lane >> 3, r = (lane >> 1) & 3, c = (lane & 1) * 4;
+    const float v0 = ch == 0 ? o[0] : ch == 1 ? o[1] : ch == 2 ? o[2] : o[3];
+    const float v1 = (ch & 1) ? o[5] : o[4];
+    for (int j = 0; j < ne; j++) {
+        const uint32_t ex = __shfl_sync(0xffffffffu, ee.x, j), ey = __shfl_sync(0xffffffffu, ee.y, j);
+        const int row = (int)(ex >> 16) * B200R_BLOCK_H + r, col = (int)(ex & 0xffffu) * B200R_BLOCK_W + c;
+        const size_t b = ey & 0x7fffffffu;
+        if (row < is && col < is) {
+            const size_t px = (size_t)row * is + col;
+            *reinterpret_cast<float4*>(soft_colors + (b * 4 + ch) * npix + px) = make_float4(v0, v0, v0, v0);
+            if (lane < 16)
+                *reinterpret_cast<float4*>(aggrs_info + (b * 2 + (ch & 1)) * npix + px) = make_float4(v1, v1, v1, v1);
+            else if (lane < 24)
+                *reinterpret_cast<int4*>(ids_out + b * P.K * npix + px) = make_int4(-1, -1, -1, -1);
+        }
+    }
+}
+
+// Empty blocks stored per shaded block, at most (<= 32: one tile_order load per lane).  Holds the whole empty list of
+// the dense workloads (C3: ~3.2 per shaded block); when the shaded blocks are few (a small object in a large image) the
+// rest goes through the queue, so that every worker shares the empty blocks and not only those holding a shaded one.
+constexpr int kFwdEmptyShare = 8;
+static_assert(kFwdEmptyShare <= kFwdLanes, "one tile_order entry per lane");
+
 template <int DIST, int RGB, bool EXACT>
 __global__ void __launch_bounds__(32, kFwdMinBlocks)
 k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const uint2* __restrict__ rects,
                   const int* __restrict__ coarse_cnt, const int* __restrict__ chunk_table,
                   const int* __restrict__ coarse_pool, const int chunks_per_bin, const float* __restrict__ textures, float* __restrict__ soft_colors,
                   float* __restrict__ aggrs_info, int* __restrict__ ids_out, int* tile_counter,
-                  const uint2* __restrict__ tile_order, float* __restrict__ pooled) {
+                  const int* __restrict__ n_empty_blocks, const uint2* __restrict__ tile_order, float* __restrict__ pooled) {
     constexpr int NT = kFwdLanes, CHUNK = kFwdChunk, UNR = kFwdUnr, TW = B200R_BLOCK_W, TH = B200R_BLOCK_H;
     constexpr unsigned FULL = 0xffffffffu;
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -356,6 +413,15 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
     const uint32_t lt_mask = (1u << lane) - 1u;
     const bool vec_out = (is & 3) == 0;
     const bool vec_ids = vec_out && ((K & 3) == 0);
+    // The queue: tile_order[0, n_shaded) holds the blocks some face rectangle touches, most expensive first, and
+    // tile_order[n_shaded, queue_len) the empty ones (cost bucket 0, k_tile_order).  When empty blocks have their
+    // constant-store path (vec_ids, no pooled epilogue), shaded entry q also stores its share of the first n_shared empty
+    // entries, [q n_shared / n_shaded, (q + 1) n_shared / n_shaded): those stores drain while the warp shades, instead of
+    // costing every worker a queue atomic and a tile_order round trip each at the end of the launch, when nothing is left
+    // to hide them behind.  The queue head skips the shared entries and hands out what the shares leave.
+    const int n_shaded = P.queue_len - *n_empty_blocks;
+    const int n_shared = (vec_ids && pooled == nullptr)
+                             ? (int)min((long long)P.queue_len - n_shaded, (long long)n_shaded * kFwdEmptyShare) : 0;
     if (lane == 0) f2_mbar_init(&S.mbar, 1);
     __syncwarp();
     uint32_t parity = 0;
@@ -366,8 +432,14 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
         int q = 0;
         if (lane == 0) q = atomicAdd(tile_counter, 1);
         q = __shfl_sync(FULL, q, 0);
-        if (q >= P.queue_len) break;
-        const uint2 te = __ldg(tile_order + q);  // most expensive blocks first (k_tile_order): x | y << 16, image | empty << 31
+        const int slot = q < n_shaded ? q : q + n_shared;
+        if (slot >= P.queue_len) break;
+        const uint2 te = __ldg(tile_order + slot);  // x | y << 16, image | empty << 31
+        if (q < n_shaded && n_shared > 0) {
+            const int e0 = (int)((long long)q * n_shared / n_shaded), ne = (int)((long long)(q + 1) * n_shared / n_shaded) - e0;
+            const uint2 ee = lane < ne ? __ldg(tile_order + n_shaded + e0 + lane) : make_uint2(0u, 0u);
+            store_empty_blocks<RGB>(ee, ne, P, softmax_sum0, soft_colors, aggrs_info, ids_out, lane);
+        }
         const int tx = (int)(te.x & 0xffffu);
         const int ty = (int)(te.x >> 16);
         const int b = (int)(te.y & 0x7fffffffu);
@@ -375,42 +447,12 @@ k_softras_forward(const SoftRasParams P, const FaceRec* __restrict__ recs, const
         const int tx0 = tx * TW, tr0 = ty * TH;   // block origin
         const int px = tx0 + lx, row = tr0 + ly;
 
-        // ---- per-pixel state, initialised as :291-309 (background buffer is all zero, Q1)
-        PixState st;
-        st.softmax_sum = softmax_sum0;
-        st.softmax_max = P.eps;
-        if (RGB == 0) { st.sc0 = st.sc1 = st.sc2 = 0.f; }
-        else if (RGB == 1) { st.sc0 = st.sc1 = st.sc2 = 0.f * softmax_sum0; }
-        else { st.sc0 = st.sc1 = st.sc2 = 1.f; }
-        st.alpha = (P.alpha_func == 2) ? 1.f : 0.f;
-        st.depth_min = 10000000.f;
-        st.face_index_min = -1;
-        st.q_size = 0;
-        st.q_max_z = -1.f;
-        st.q_max_id = -1;
-
-        // ---- blocks no rectangle touches (78 % of the blocks at C3): every pixel leaves with its initial state.  Six constant
-        // planes and the terminator of the id lists, straight from registers.
+        // ---- empty blocks the shares left to the queue (all of them when no block of the batch is shaded)
         if (empty && vec_ids && pooled == nullptr) {
-            float o[6];
-            finalize_pixel<RGB>(st, P, o[0], o[1], o[2], o[3], o[4], o[5]);
-            for (int j = lane; j < 6 * TH * 2; j += NT) {
-                const int ch = j >> 3, r = (j >> 1) & 3, q = j & 1;
-                const float v = ch == 0 ? o[0] : ch == 1 ? o[1] : ch == 2 ? o[2] : ch == 3 ? o[3] : ch == 4 ? o[4] : o[5];
-                const int orow = tr0 + r, ocol = tx0 + q * 4;
-                if (orow < is && ocol < is) {
-                    float* dst = (ch < 4) ? soft_colors + ((size_t)b * 4 + ch) * npix
-                                          : aggrs_info + ((size_t)b * 2 + (ch - 4)) * npix;
-                    *reinterpret_cast<float4*>(dst + (size_t)orow * is + ocol) = make_float4(v, v, v, v);
-                }
-            }
-            if (lane < TH * 2) {
-                const int orow = tr0 + (lane >> 1), ocol = tx0 + (lane & 1) * 4;
-                if (orow < is && ocol < is)
-                    *reinterpret_cast<int4*>(ids_out + (size_t)b * K * npix + (size_t)orow * is + ocol) = make_int4(-1, -1, -1, -1);
-            }
+            store_empty_blocks<RGB>(te, 1, P, softmax_sum0, soft_colors, aggrs_info, ids_out, lane);
             continue;
         }
+        PixState st = initial_state<RGB>(P, softmax_sum0);
 
         const float xp = b200r_pix_coord(px, is);
         const float yp = b200r_pix_coord(is - 1 - row, is);

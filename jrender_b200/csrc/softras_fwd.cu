@@ -43,7 +43,7 @@ int launch_forward(const SoftRasParams& P, const SoftRasWorkspace& W, const floa
     return b200r_launch("k_softras_forward", B200R_K_SOFTRAS_FWD, k_softras_forward<DIST, RGB, EXACT>,
                         dim3((unsigned)(total < slots ? total : slots), 1), 32, smem, st, P, W.recs, W.rects, W.coarse_cnt,
                         W.chunk_table, W.coarse_pool, W.chunks_per_bin, textures, soft_colors, aggrs_info, ids, W.counters,
-                        W.tile_order, pooled);
+                        W.counters + 64, W.tile_order, pooled);   // counters[64] = cost bucket 0: the empty blocks
 }
 
 }  // namespace

@@ -434,7 +434,9 @@ static __global__ void __launch_bounds__(256) k_coarse_bin(const uint2* __restri
 // persistent raster grid): each queue entry takes the bucket of its own block's cost (k_coarse_bin),
 // so a silhouette block that is long-running starts early even when its neighbours are cheap.
 // hist[] counts blocks per bucket (complete after k_coarse_bin).  Block-aggregated reservation:
-// one global atomic per (CTA, bucket) instead of one per block.
+// one global atomic per (CTA, bucket) instead of one per block.  Bucket 0 (no rectangle touches the block) comes last:
+// tile_order[0, total - hist[0]) are the blocks with faces to shade, tile_order[total - hist[0], total) the empty
+// ones, which k_softras_forward stores on the side of the shaded blocks.
 static __global__ void __launch_bounds__(256) k_tile_order(const int* __restrict__ tile_cost, const int* __restrict__ hist,
                                                            int* __restrict__ cursor, uint2* __restrict__ tile_order,
                                                            int B, int fntx, int fnty) {
