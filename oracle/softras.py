@@ -51,6 +51,14 @@ def lib():
             C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_float, C.c_float,
             C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
             f32p, C.POINTER(C.c_int64), C.c_long]
+        _lib.softras_oracle_forward_bound.restype = None
+        _lib.softras_oracle_forward_bound.argtypes = [
+            f32p, f32p, f32p, f32p, f32p, i32p,
+            C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+            C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_float, C.c_float,
+            C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+            C.POINTER(C.c_double), C.POINTER(C.c_double), i32p, C.POINTER(C.c_uint32),
+            C.c_int, C.c_int, C.c_int, C.c_int]
         _lib.softras_oracle_max_threads.restype = C.c_int
     return _lib
 
@@ -103,6 +111,46 @@ def forward(face_vertices, textures, params, rows=None, nthreads=0, row_stride=1
         _p(fv, C.c_float), _p(tx, C.c_float), _p(faces_info, C.c_float), _p(aggrs_info, C.c_float),
         _p(soft_colors, C.c_float), _p(ids, C.c_int32), B, nf, T, H, K, *params.scalars(), r0, r1, int(row_stride), nthreads)
     return dict(soft_colors=soft_colors, faces_info=faces_info, aggrs_info=aggrs_info, faces_id_buffer=ids)
+
+
+# softras_oracle.c's rounding sites, by bit of forward_bound's `live`
+SITES = ["exp_sig", "exp_soft", "tail_d", "prod", "div_sigarg", "div_zsoft", "div_cold", "div_gamma", "div_nmf",
+         "div_sigma"] + ["div_%s%d" % (n, k) for n in ("z1_", "z2_", "clipw", "clipz", "euc") for k in range(3)] + \
+        ["exp_bg", "div_span"]
+SITE = {n: i for i, n in enumerate(SITES)}
+MARG_ALPHA, MARG_MAX = 1, 2   # forward_bound's `marginal` bits
+
+
+def site_names(mask):
+    return [n for i, n in enumerate(SITES) if int(mask) >> i & 1]
+
+
+def forward_bound(face_vertices, textures, params, exact_tail=False, nudge=0, rows=None, row_stride=1, nthreads=0):
+    """forward() plus the CUDA forward's error bound per output entry (softras_oracle.c, "rounding sites of the K2
+    forward").  Adds bound_colors [B,4,H,W] (on |CUDA soft_colors - oracle|), bound_sum [B,H,W] (on the softmax sum,
+    aggrs_info[:, 0]; 0 where that channel is not the sum), marginal [B,H,W] (MARG_* bits: a decision the error can
+    flip; those entries' bounds are inf) and live [B,H,W] (bit SITE[name]: the site was live in one of the pixel's
+    pairs).  exact_tail: the kernel's softras_exact_tail.  nudge = +1 / -1 / >= 2: the outputs are the forward with every
+    live site moved by its budget up / down / by a hashed sign, the hash seeded by nudge - 2 for nudge >= 2 (and,
+    without exact_tail, the kernel's fp32 tails)."""
+    fv = np.ascontiguousarray(face_vertices, dtype=np.float32)
+    tx = np.ascontiguousarray(textures, dtype=np.float32)
+    B, nf = fv.shape[:2]
+    T = tx.shape[2]
+    H = int(params["image_size"])
+    K = int(params["max_faces_per_pixel_for_grad"])
+    assert K <= 64
+    out = dict(faces_info=np.zeros((B, nf, 27), np.float32), aggrs_info=np.zeros((B, 2, H, H), np.float32),
+               soft_colors=np.zeros((B, 4, H, H), np.float32), faces_id_buffer=np.zeros((B, K, H, H), np.int32),
+               bound_colors=np.zeros((B, 4, H, H)), bound_sum=np.zeros((B, H, H)),
+               marginal=np.zeros((B, H, H), np.int32), live=np.zeros((B, H, H), np.uint32))
+    r0, r1 = (0, H) if rows is None else rows
+    lib().softras_oracle_forward_bound(
+        _p(fv, C.c_float), _p(tx, C.c_float), _p(out["faces_info"], C.c_float), _p(out["aggrs_info"], C.c_float),
+        _p(out["soft_colors"], C.c_float), _p(out["faces_id_buffer"], C.c_int32), B, nf, T, H, K, *params.scalars(),
+        int(bool(exact_tail)), int(nudge), _p(out["bound_colors"], C.c_double), _p(out["bound_sum"], C.c_double),
+        _p(out["marginal"], C.c_int32), _p(out["live"], C.c_uint32), r0, r1, int(row_stride), nthreads)
+    return out
 
 
 def backward(face_vertices, textures, fwd, grad_soft_colors, params, accumulate_double=True, rows=None, row_stride=1,

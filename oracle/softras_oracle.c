@@ -77,7 +77,10 @@ enum {
     SITE_DIV_CLIPW = SITE_DIV_Z2 + 3,   /* + k: w_k / w_sum */
     SITE_DIV_CLIPZ = SITE_DIV_CLIPW + 3, /* + k: w_k / z_k inside zp */
     SITE_DIV_EUC = SITE_DIV_CLIPZ + 3,  /* + k: the euclidean edge parameter of edge k */
-    N_SITES = SITE_DIV_EUC + 3
+    N_SITES = SITE_DIV_EUC + 3,
+    /* forward only (see "rounding sites of the K2 forward" below) */
+    SITE_EXP_BG = N_SITES, SITE_DIV_SPAN,
+    N_FWD_SITES
 };
 typedef struct {
     int exact_tail;       /* the kernel's softras_exact_tail */
@@ -350,6 +353,137 @@ typedef struct {
     float z;
 } Pixel; /* :238-241 */
 
+/* ------------------------------------------------------------------ rounding sites of the K2 forward
+ * The CUDA forward (softras_forward.cuh shade_face / aggregate_alpha / initial_state / finalize_pixel, with DivPolicy
+ * of softras_math.cuh) evaluates every discrete decision of a pixel -- border, inside, distance threshold, zp, near /
+ * far, top-K, the nearest face -- with this file's arithmetic bit for bit: its euclidean edge parameter, clip and zp
+ * divisions and the vertex-texture divisions are strict (correctly rounded for every input), and finalize_pixel's
+ * colour quotients are fast_div (correctly rounded too).  It may differ only at these sites:
+ *   SITE_EXP_BG     expf(eps / gamma), the initial softmax_sum: <= 3 ulp, as SITE_EXP_SIG of the backward.
+ *   SITE_EXP_SIG    expf in the sigmoid: <= 3 ulp.
+ *   SITE_EXP_SOFT   expf of exp_delta_zp and of exp_z: <= 3 ulp.  expf(+-0) is 1 exactly in both libraries, so a site
+ *                   whose argument is zero (exp_z of the face that raised softmax_max; the OPT body sets that weight to
+ *                   1 without an expf) is not live.
+ *   SITE_TAIL_D     softras_exact_tail = 0: D = rcp(1.f + e), two fp32 roundings (rcp is IEEE 1 / y), where this file
+ *                   rounds the double quotient once.
+ *   SITE_PROD       softras_exact_tail = 0: alpha * (1.f - D) in fp32, where this file rounds the double product once
+ *                   (the same bits when D is exactly 0 or 1, as under hard distances).
+ *   SITE_DIV_SIGARG softras_exact_tail = 0: by_sigma(-sign * dis), a relaxed division: exact for numerators >= 2^-60
+ *                   and within 1 ulp below (exact_math.cuh relaxed_div; the slow path when sigma is not midrange).
+ *   SITE_DIV_SPAN   softras_exact_tail = 0: by_span(far - zp), likewise; it feeds zp_norm, softmax_max and the
+ *                   `zp_norm > softmax_max` decision.
+ *   SITE_DIV_GAMMA  softras_exact_tail = 0: by_gamma of the two exp arguments, likewise.
+ * With softras_exact_tail = 1 the tails and divisions are the reference's bit for bit: only the expf sites remain.
+ *
+ * The bound.  Beside each state variable of a pixel (softmax_sum, sc0..2, alpha, softmax_max) the forward carries an
+ * interval [lo, hi] in float that holds every value the kernel can have there.  An expf site widens its value by its
+ * budget: the libm expf of each end moved 3 ulp outwards.  That needs no monotone libm: CUDA's expf is within 2 ulp of
+ * exp and libm's within 1, and exp itself is monotone, so for any x' in [lo, hi] the kernel's expf(x') is at least
+ * exp(lo) - 2 ulp >= expf_libm(lo) - 3 ulp, and at most expf_libm(hi) + 3 ulp likewise; a division
+ * site widens the quotient by 1 ulp whenever the numerator's interval reaches a non-zero value below 2^-60; the tail
+ * sites are the kernel's own fp32 expressions, evaluated on the interval's ends.  Every update the pixel makes
+ * (s' = a s + b c, the exp_delta_zp rescale, 1 - alpha, / nf, sc / softmax_sum) is monotone in each operand once the
+ * operands' signs are fixed, and rounding to nearest is monotone, so evaluating the kernel's float operations on the
+ * corners of the operand intervals (min and max of the four products, ends of sums) encloses the kernel's result --
+ * this is at least as tight as adding |x - y| + ulp(x) / 2 + ulp(y) / 2 per operation.  The bound of an output is its
+ * interval's largest distance from this file's value.  Zero stays zero: an interval that never met a live site is the
+ * single value this file computes, so its bound is exactly 0 and the kernel must match it bit for bit.
+ *
+ * Decisions that read a widened value: hard alpha's `D > 0.5` and `zp_norm > softmax_max`.  Where the decision's
+ * interval straddles the threshold the pixel is marginal: FWD_MARG_ALPHA (its alpha's bound is infinite) or
+ * FWD_MARG_MAX (its colours' and softmax_sum's bounds are infinite; softmax_max is bit-exact only where no
+ * SITE_DIV_SPAN is live).  Near / far and the top-K read zp, which is exact, so they never are.
+ *
+ * Nudging (FwdBound.nudge = +1 / -1 / >= 2): every live expf and division site moved by its budget up / down / by a
+ * hashed sign per (pixel, face, site; the hash seeded by nudge - 2), and, with exact_tail = 0, the tails taken in the kernel's fp32 form: a forward
+ * the kernel could have computed, which must stay within the bound of the plain one. */
+enum { FWD_MARG_ALPHA = 1, FWD_MARG_MAX = 2 };
+typedef struct {
+    int exact_tail;                    /* the kernel's softras_exact_tail */
+    int nudge;                         /* 0, +1, -1, >= 2 (above) */
+    double *bound_colors, *bound_sum;  /* [B,4,H,W], [B,H,W] */
+    int32_t *marginal;                 /* [B,H,W] FWD_MARG_* */
+    uint32_t *live;                    /* [B,H,W] bit s: site s was live in one of the pixel's pairs */
+} FwdBound;
+
+typedef struct {
+    float lo, hi;
+} Iv;
+static inline Iv iv(float x) { Iv r = {x, x}; return r; }
+static inline Iv iv2(float a, float b) {   /* NaN anywhere: the NaN interval */
+    if (isnan(a) || isnan(b)) return iv(NAN);
+    Iv r = {fminf(a, b), fmaxf(a, b)};
+    return r;
+}
+static inline Iv iv4(float a, float b, float c, float d) {
+    const Iv x = iv2(a, b), y = iv2(c, d);
+    return iv2(fminf(x.lo, y.lo), fmaxf(x.hi, y.hi));
+}
+static inline int iv_point(Iv a) { return a.lo == a.hi; }
+static inline Iv iv_add(Iv a, Iv b) { return iv2(a.lo + b.lo, a.hi + b.hi); }
+static inline Iv iv_mul(Iv a, Iv b) { return iv4(a.lo * b.lo, a.lo * b.hi, a.hi * b.lo, a.hi * b.hi); }
+static inline Iv iv_div(Iv a, Iv b) {
+    if (iv_point(a) && iv_point(b)) return iv(a.lo / b.lo);
+    if (!(b.lo > 0.f || b.hi < 0.f)) return iv2(-INFINITY, INFINITY);
+    return iv4(a.lo / b.lo, a.lo / b.hi, a.hi / b.lo, a.hi / b.hi);
+}
+static inline float move_fin(float x, int n, int dir) { return isfinite(x) ? move_ulps(x, n, dir) : x; }
+static inline float clamp0(float x) { return x < 0.f ? 0.f : x; }   /* NaN stays NaN */
+
+/* |kernel - this file's value o| over the interval; 0 exactly for the point interval {o} */
+static inline double iv_bound(float o, Iv r) {
+    if (iv_point(r) && (r.lo == o || (isnan(r.lo) && isnan(o)))) return 0.0;
+    const double b = fmax((double)r.hi - (double)o, (double)o - (double)r.lo);
+    return isnan(b) ? INFINITY : b;
+}
+
+/* the sigmoid tail, D = 1 / (1 + e): the reference's double quotient, or the kernel's fp32 one */
+static inline float tail_d(float e, int fp32) { return fp32 ? 1.f / (1.f + e) : (float)(1. / (1. + (double)e)); }
+/* alpha "prod": alpha * (1 - D), likewise */
+static inline float tail_prod(float a, float D, int fp32) {
+    return fp32 ? a * (1.f - D) : (float)((double)a * (1. - (double)D));
+}
+
+/* a / b as a relaxed division of the kernel (by_sigma, by_span, by_gamma): returns this file's (possibly nudged) a / b
+ * and sets *qi to the interval of the kernel's quotient for a numerator anywhere in ai */
+static float fwd_rdiv(Nudge *nd, int s, float a, Iv ai, float b, Iv *qi) {
+    float q = a / b;
+    if (!nd) return q;
+    *qi = iv2(ai.lo / b, ai.hi / b);
+    if (!nd->exact_tail && fabsf(b) >= 0x1p-60f && fabsf(b) < 0x1p61f && ai.lo < 0x1p-60f && ai.hi > -0x1p-60f &&
+        !(ai.lo == 0.f && ai.hi == 0.f)) {
+        nd->live |= 1u << s;
+        qi->lo = move_fin(qi->lo, 1, -1);
+        qi->hi = move_fin(qi->hi, 1, 1);
+        if (a != 0.f && fabsf(a) < 0x1p-60f) q = site(nd, s, q, 1);
+    }
+    return q;
+}
+
+/* expf(x) at site s for x in xi: returns this file's (possibly nudged) value, *ei the kernel's interval */
+static float fwd_exp(Nudge *nd, int s, float x, Iv xi, Iv *ei) {
+    float e = expf(x);
+    if (!nd) return e;
+    if (xi.lo == 0.f && xi.hi == 0.f) {
+        *ei = iv(1.f);
+        return e;
+    }
+    *ei = iv2(clamp0(move_fin(expf(xi.lo), 3, -1)), move_fin(expf(xi.hi), 3, 1));
+    return clamp0(site(nd, s, e, 3));
+}
+
+/* soft_fragment = 1. / (1. + exp(num / sigma)) (:338, :344); *Di the kernel's interval */
+static float fwd_sigmoid(Nudge *nd, const FwdBound *fb, float num, float sigma_val, Iv *Di) {
+    if (!nd) return (float)(1. / (1. + (double)expf(num / sigma_val)));
+    Iv xi, ei;
+    const float x = fwd_rdiv(nd, SITE_DIV_SIGARG, num, iv(num), sigma_val, &xi);
+    const float e = fwd_exp(nd, SITE_EXP_SIG, x, xi, &ei);
+    const int fp32 = !fb->exact_tail;
+    if (fp32) nd->live |= 1u << SITE_TAIL_D;
+    *Di = iv2(tail_d(ei.hi, fp32), tail_d(ei.lo, fp32));
+    return tail_d(e, fp32 && fb->nudge);
+}
+
 /* ------------------------------------------------------------------ K2 :243-456
  * Processes output rows row_begin, row_begin+row_stride, ... < row_end of every batch
  * element (row 0 = top); the full op is row_begin=0, row_end=image_size, row_stride=1.  Buffers must be pre-initialised
@@ -360,7 +494,8 @@ static void forward_rows(const float *faces, const float *textures, const float 
                          int texture_size, int texture_res, float near, float far, float eps,
                          float sigma_val, int func_id_dist, float dist_eps, float gamma_val,
                          int func_id_rgb, int func_id_alpha, int texture_sample_type,
-                         int double_side, int row_begin, int row_end, int row_stride, int nthreads) {
+                         int double_side, int row_begin, int row_end, int row_stride, int nthreads,
+                         const FwdBound *fb) {
     const int is = image_size;
     const int nf = num_faces;
     const long npix = (long)is * is;
@@ -399,14 +534,26 @@ static void forward_rows(const float *faces, const float *textures, const float 
             const float *face_info = &faces_info[(long)bn * nf * 27] - 27;
             const float *fbb = &bb[(long)bn * nf * 4] - 4;
 
+            /* fb: the kernel's intervals beside the state (see "rounding sites of the K2 forward") */
+            Nudge nd = {fb ? fb->exact_tail : 1, 0, 0, fb && fb->nudge >= 2, 0, 0};
+            if (fb && fb->nudge == 1) nd.up = ~0u;
+            if (fb && fb->nudge == -1) nd.down = ~0u;
+            Nudge *ndp = fb ? &nd : NULL;
+            int marg = 0;
+
             float soft_color[4] = {1.f, 1.f, 1.f, 0.f};
             if (func_id_alpha == 2) soft_color[3] = 1.f;
-            float softmax_sum = expf(eps / gamma_val);
+            Iv sumi = iv(0.f), smi = iv(eps), sci[4];
+            const float softmax_sum0 = eps / gamma_val;
+            float softmax_sum = func_id_rgb == 1 ? fwd_exp(ndp, SITE_EXP_BG, softmax_sum0, iv(softmax_sum0), &sumi)
+                                                 : expf(softmax_sum0);
             float softmax_max = eps;
             for (int k = 0; k < 3; k++) {
                 if (func_id_rgb == 0) soft_color[k] = soft_colors[((long)bn * 4 + k) * npix + pn];
                 else if (func_id_rgb == 1) soft_color[k] = soft_colors[((long)bn * 4 + k) * npix + pn] * softmax_sum;
+                if (fb) sci[k] = iv_mul(iv(soft_colors[((long)bn * 4 + k) * npix + pn]), sumi);
             }
+            sci[3] = iv(soft_color[3]);   /* (the intervals are only read when fb is set) */
             float depth_min = 10000000;
             int face_index_min = -1;
             Pixel q[K_MAX_POINTS_PER_PIXEL];
@@ -423,6 +570,9 @@ static void forward_rows(const float *faces, const float *textures, const float 
                 if (xp > fbb[0] || xp < fbb[1] || yp > fbb[2] || yp < fbb[3]) continue; /* :316 */
 
                 float dis, dis_x, dis_y, t[3], w[3], w_clip[3], sign, soft_fragment;
+                Iv Di = iv(1.f);
+                nd.pair = (uint32_t)(((long)bn * npix + pn) * 0x9E3779B1u) ^ (uint32_t)fn * 0x85EBCA77u ^
+                          (uint32_t)(fb && fb->nudge > 2 ? fb->nudge : 0) * 0x27D4EB2Fu;
 
                 barycentric_coordinate(w, xp, yp, face_info);
 
@@ -432,20 +582,31 @@ static void forward_rows(const float *faces, const float *textures, const float 
                 } else if (func_id_dist == 1) {
                     dis = forward_barycentric_p2f_distance(w);
                     if (-dis >= threshold) continue;
-                    soft_fragment = (float)(1. / (1. + (double)expf(-dis / sigma_val)));
+                    soft_fragment = fwd_sigmoid(ndp, fb, -dis, sigma_val, &Di);
                 } else {
                     euclidean_p2f_distance(&sign, &dis_x, &dis_y, w, t, face, face_info, xp, yp, NULL);
                     dis = dis_x * dis_x + dis_y * dis_y;
                     if (sign < 0 && dis >= threshold) continue;
-                    soft_fragment = (float)(1. / (1. + (double)expf(-sign * dis / sigma_val)));
+                    soft_fragment = fwd_sigmoid(ndp, fb, -sign * dis, sigma_val, &Di);
                 }
 
                 if (func_id_alpha == 0) {
                     if (soft_fragment > 0.5) soft_color[3] = 1.f;
+                    if (fb) {
+                        if (Di.hi > 0.5f) sci[3].hi = 1.f;
+                        if (Di.lo > 0.5f) sci[3].lo = 1.f;
+                        if (!iv_point(Di) && Di.lo <= 0.5f && Di.hi > 0.5f) marg |= FWD_MARG_ALPHA;
+                    }
                 } else if (func_id_alpha == 1) {
                     soft_color[3] += soft_fragment;
+                    if (fb) sci[3] = iv_add(sci[3], Di);
                 } else if (func_id_alpha == 2) {
-                    soft_color[3] = (float)((double)soft_color[3] * (1. - (double)soft_fragment));
+                    const int fp32 = fb && !fb->exact_tail;
+                    soft_color[3] = tail_prod(soft_color[3], soft_fragment, fp32 && fb->nudge);
+                    if (fp32 && !(iv_point(Di) && (Di.lo == 0.f || Di.lo == 1.f))) nd.live |= 1u << SITE_PROD;   /* else exact */
+                    if (fb)
+                        sci[3] = iv4(tail_prod(sci[3].lo, Di.lo, fp32), tail_prod(sci[3].lo, Di.hi, fp32),
+                                     tail_prod(sci[3].hi, Di.lo, fp32), tail_prod(sci[3].hi, Di.hi, fp32));
                 }
 
                 for (int k = 0; k < 3; k++) w_clip[k] = w[k];
@@ -478,22 +639,37 @@ static void forward_rows(const float *faces, const float *textures, const float 
                     if (zp < depth_min && check_pixel_inside(w) && (double_side || check_face_frontside(face))) {
                         depth_min = zp;
                         face_index_min = fn;
-                        for (int k = 0; k < 3; k++)
+                        for (int k = 0; k < 3; k++) {
                             soft_color[k] = forward_sample_texture_fwd(texture, w_clip, texture_res, k, texture_sample_type, face, zp);
+                            if (fb) sci[k] = iv(soft_color[k]);
+                        }
                     }
                 } else if (func_id_rgb == 1) {
                     if (check_face_frontside(face) || double_side) {
-                        const float zp_norm = (far - zp) / (far - near);
+                        Iv zni = iv(0.f), qi = iv(0.f), edi = iv(1.f), ezi = iv(1.f);
+                        const float zp_norm = fwd_rdiv(ndp, SITE_DIV_SPAN, far - zp, iv(far - zp), far - near, &zni);
                         float exp_delta_zp = 1.f;
-                        if (zp_norm > softmax_max) {
-                            exp_delta_zp = expf((softmax_max - zp_norm) / gamma_val);
+                        const int up = zp_norm > softmax_max;
+                        if (fb && !(iv_point(zni) && iv_point(smi)) && (up ? !(zni.lo > smi.hi) : !(zni.hi <= smi.lo)))
+                            marg |= FWD_MARG_MAX;
+                        if (up) {
+                            const float q = fwd_rdiv(ndp, SITE_DIV_GAMMA, softmax_max - zp_norm,
+                                                     fb ? iv2(smi.lo - zni.hi, smi.hi - zni.lo) : qi, gamma_val, &qi);
+                            exp_delta_zp = fwd_exp(ndp, SITE_EXP_SOFT, q, qi, &edi);
                             softmax_max = zp_norm;
+                            smi = zni;
                         }
-                        const float exp_z = expf((zp_norm - softmax_max) / gamma_val);
+                        const float q = fwd_rdiv(ndp, SITE_DIV_GAMMA, zp_norm - softmax_max,
+                                                 !fb ? qi : up ? iv(zp_norm - softmax_max) : iv2(zni.lo - smi.hi, zni.hi - smi.lo),
+                                                 gamma_val, &qi);
+                        const float exp_z = fwd_exp(ndp, SITE_EXP_SOFT, q, qi, &ezi);
                         softmax_sum = exp_delta_zp * softmax_sum + exp_z * soft_fragment;
+                        const Iv wi = fb ? iv_mul(ezi, Di) : ezi;
+                        if (fb) sumi = iv_add(iv_mul(edi, sumi), wi);
                         for (int k = 0; k < 3; k++) {
                             const float color_k = forward_sample_texture_fwd(texture, w_clip, texture_res, k, texture_sample_type, face, zp);
                             soft_color[k] = exp_delta_zp * soft_color[k] + exp_z * soft_fragment * color_k;
+                            if (fb) sci[k] = iv_add(iv_mul(edi, sci[k]), iv_mul(wi, iv(color_k)));
                         }
                     }
                 }
@@ -503,6 +679,22 @@ static void forward_rows(const float *faces, const float *textures, const float 
             if (func_id_alpha == 0) soft_colors[((long)bn * 4 + 3) * npix + pn] = soft_color[3];
             else if (func_id_alpha == 1) soft_colors[((long)bn * 4 + 3) * npix + pn] = soft_color[3] / nf;
             else if (func_id_alpha == 2) soft_colors[((long)bn * 4 + 3) * npix + pn] = (float)(1. - (double)soft_color[3]);
+            if (fb) {
+                Iv ai = sci[3];
+                if (func_id_alpha == 1) ai = iv2(ai.lo / nf, ai.hi / nf);
+                else if (func_id_alpha == 2) ai = iv2((float)(1. - (double)ai.hi), (float)(1. - (double)ai.lo));
+                const long o = (long)bn * npix + pn;
+                for (int k = 0; k < 3; k++) {
+                    double b = 0.0;
+                    if (func_id_rgb == 1) b = (marg & FWD_MARG_MAX) ? INFINITY : iv_bound(soft_color[k] / softmax_sum, iv_div(sci[k], sumi));
+                    fb->bound_colors[((long)bn * 4 + k) * npix + pn] = b;
+                }
+                fb->bound_colors[((long)bn * 4 + 3) * npix + pn] =
+                    (marg & FWD_MARG_ALPHA) ? INFINITY : iv_bound(soft_colors[((long)bn * 4 + 3) * npix + pn], ai);
+                fb->bound_sum[o] = func_id_rgb != 1 ? 0.0 : (marg & FWD_MARG_MAX) ? INFINITY : iv_bound(softmax_sum, sumi);
+                fb->marginal[o] = marg;
+                fb->live[o] = nd.live;
+            }
 
             if (func_id_rgb == 0) {
                 if (face_index_min != -1)
@@ -539,7 +731,37 @@ void softras_oracle_forward(const float *faces, const float *textures, float *fa
     forward_rows(faces, textures, faces_info, aggrs_info, soft_colors, faces_id_buffer, batch_size,
                  num_faces, image_size, max_faces_id, texture_size, texture_res, near, far, eps,
                  sigma_val, func_id_dist, dist_eps, gamma_val, func_id_rgb, func_id_alpha,
-                 texture_sample_type, double_side, row_begin, row_end, row_stride, nthreads);
+                 texture_sample_type, double_side, row_begin, row_end, row_stride, nthreads, NULL);
+}
+
+/* softras_oracle_forward with the kernel's error bound per output entry ("rounding sites of the K2 forward"):
+ * bound_colors [B,4,H,W] on |CUDA soft_colors - this file's|, bound_sum [B,H,W] on softmax_sum (aggrs_info channel 0;
+ * 0 where it is not the softmax sum), marginal [B,H,W] FWD_MARG_* bits, live [B,H,W] the sites live in the pixel.
+ * exact_tail: the kernel's softras_exact_tail.  nudge != 0: the outputs are the nudged forward (the bounds then mean
+ * nothing).  Rows outside row_begin + i row_stride keep the memsets' values and bound 0. */
+void softras_oracle_forward_bound(const float *faces, const float *textures, float *faces_info,
+                                  float *aggrs_info, float *soft_colors, int32_t *faces_id_buffer,
+                                  int batch_size, int num_faces, int texture_size, int image_size,
+                                  int max_faces_id, float near, float far, float eps, float sigma_val,
+                                  int func_id_dist, float dist_eps, float gamma_val, int func_id_rgb,
+                                  int func_id_alpha, int texture_sample_type, int double_side, int exact_tail,
+                                  int nudge, double *bound_colors, double *bound_sum, int32_t *marginal,
+                                  uint32_t *live, int row_begin, int row_end, int row_stride, int nthreads) {
+    const size_t npix = (size_t)image_size * image_size;
+    memset(aggrs_info, 0, sizeof(float) * 2 * npix * batch_size);
+    memset(soft_colors, 0, sizeof(float) * 4 * npix * batch_size);
+    memset(faces_id_buffer, 0xFF, sizeof(int32_t) * (size_t)max_faces_id * npix * batch_size);
+    memset(bound_colors, 0, sizeof(double) * 4 * npix * batch_size);
+    memset(bound_sum, 0, sizeof(double) * npix * batch_size);
+    memset(marginal, 0, sizeof(int32_t) * npix * batch_size);
+    memset(live, 0, sizeof(uint32_t) * npix * batch_size);
+    softras_oracle_face_info(faces, faces_info, batch_size, num_faces);
+    const int texture_res = (int)sqrt((double)texture_size);
+    const FwdBound fb = {exact_tail, nudge, bound_colors, bound_sum, marginal, live};
+    forward_rows(faces, textures, faces_info, aggrs_info, soft_colors, faces_id_buffer, batch_size,
+                 num_faces, image_size, max_faces_id, texture_size, texture_res, near, far, eps,
+                 sigma_val, func_id_dist, dist_eps, gamma_val, func_id_rgb, func_id_alpha,
+                 texture_sample_type, double_side, row_begin, row_end, row_stride, nthreads, &fb);
 }
 
 /* ------------------------------------------------------------------ K6 :1177-1360

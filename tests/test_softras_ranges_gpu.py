@@ -279,7 +279,7 @@ def both_tails(fv, tex, P, **kw):
     try:
         for tail in (0, 1):
             _lib.set_option("softras_exact_tail", tail)
-            check(fv, tex, P, nan=True, **kw)
+            check(fv, tex, P, nan=True, exact_tail=bool(tail), **kw)
     finally:
         _lib.set_option("softras_exact_tail", 0)
 
@@ -304,7 +304,7 @@ def test_non_finite_vertices_stay_in_their_batch_element(cuda_device, dist):
     try:
         for tail in (0, 1):
             _lib.set_option("softras_exact_tail", tail)
-            check(bad, tex, P, nan=True)
+            check(bad, tex, P, nan=True, exact_tail=bool(tail))
             got, base = run_cuda(bad, tex, P, grad=g), run_cuda(clean, tex, P, grad=g)
             for k in ("soft_colors", "aggrs_info", "faces_id_buffer", "faces_info"):
                 assert np.array_equal(got[k][0], base[k][0]), k

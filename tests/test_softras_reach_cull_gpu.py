@@ -91,7 +91,7 @@ def both_tails(fv, tex, P, nan=False):
     try:
         for tail in (0, 1):
             _lib.set_option("softras_exact_tail", tail)
-            check(fv, tex, P, nan=nan)
+            check(fv, tex, P, nan=nan, exact_tail=bool(tail))
     finally:
         _lib.set_option("softras_exact_tail", 0)
 

@@ -66,6 +66,86 @@ def backward_bound_ratio(got, fv, tex, params, grad, exact_tail=False, row_strid
     return worst
 
 
+def same_nonfinite(a, b, what):
+    """NaN, +inf and -inf in the same places of a and b; returns the mask of b's finite entries."""
+    assert np.array_equal(np.isnan(a), np.isnan(b)), "%s NaN pattern differs" % what
+    assert np.array_equal(np.isposinf(a), np.isposinf(b)) and np.array_equal(np.isneginf(a), np.isneginf(b)), what
+    return np.isfinite(b)
+
+
+def hold_to_bound(a, ref, bound, what, live=None):
+    """Every finite entry of a within its bound of ref, bit-equal where the bound is 0, NaN / inf where ref has them.
+    live ([B,H,W] site bits, None): named in the failure message.  -> (worst |a - ref| / bound, entries with bound > 0)."""
+    m = same_nonfinite(a, ref, what)
+    eq0 = (bound == 0) & m
+    a32, r32 = np.ascontiguousarray(a, np.float32), np.ascontiguousarray(ref, np.float32)
+    diff0 = eq0 & (a32.view(np.uint32) != r32.view(np.uint32))
+    err = np.where(m, np.abs(a.astype(np.float64) - ref.astype(np.float64)), 0.0)
+    bad = diff0 | (m & ~(err <= bound))
+    if bad.any():
+        ratio = np.where(bad, err / np.where(bound > 0, bound, 1e-300), 0.0)
+        idx = np.unravel_index(int(np.argmax(np.where(diff0, np.inf, ratio))), a.shape)
+        sites = "" if live is None else " live sites %s" % osr.site_names(live[(idx[0],) + tuple(idx[-2:])])
+        raise AssertionError("%s: %d entries outside the forward bound; worst at %s: got %r, oracle %r, bound %r%s" % (
+            what, int(bad.sum()), idx, float(a[idx]), float(ref[idx]), float(bound[idx]), sites))
+    pos = m & (bound > 0)
+    return float((err[pos] / bound[pos]).max(initial=0.0)), int(pos.sum())
+
+
+def forward_bound_ratio(got, fv, tex, params, exact_tail=False, row_stride=1, ref=None, nan=False):
+    """Holds the SoftRas forward's float outputs of `got` (run_cuda) to the oracle, entry by entry: soft_colors and the
+    softmax sum (aggrs_info[:, 0]) within osr.forward_bound's per-entry bound (bit-equal where it is 0: no rounding
+    site live), softmax_max and the hard-mode aggregates bit-exact.  nan=False: no NaN in any of these outputs;
+    nan=True (inputs on which the reference's own arithmetic yields NaN): NaN / inf where the oracle's are.
+    exact_tail: the kernel's softras_exact_tail; each setting has its own bound, since the two tails round
+    differently.  row_stride: compare rows 0, row_stride, ... only.  ref: osr.forward_bound's result for these inputs,
+    if already computed.
+    -> dict(colors=(worst err / bound, entries with a non-zero bound), sum=(...), ref=the oracle's outputs)."""
+    H = int(params["image_size"])
+    # the forward takes the fp32 tails in euclidean mode only; the other distances always run the exact tails
+    # (softras_fwd.cu b200r_launch_forward)
+    exact_tail = exact_tail or params["dist_func"] != "euclidean"
+    if ref is None:
+        ref = osr.forward_bound(fv, tex, params, exact_tail=exact_tail, row_stride=row_stride)
+    rows = np.arange(0, H, row_stride)
+    sc, ag = got["soft_colors"][:, :, rows], got["aggrs_info"][:, :, rows]
+    if not nan:
+        assert not np.isnan(sc).any(), "NaN in soft_colors"
+        assert not np.isnan(ag).any(), "NaN in aggrs_info"
+    live = ref["live"][:, rows]
+    res = dict(ref=ref)
+    res["colors"] = hold_to_bound(sc, ref["soft_colors"][:, :, rows], ref["bound_colors"][:, :, rows], "soft_colors", live)
+    if params["aggr_func_rgb"] == "softmax":
+        marg = ref["marginal"][:, rows]
+        same = (ag[:, 1] == ref["aggrs_info"][:, 1, rows]) | (np.isnan(ag[:, 1]) & np.isnan(ref["aggrs_info"][:, 1, rows]))
+        assert same.all(), "softmax_max not bit-exact (%d entries, %d of them at pixels with a marginal decision)" % (
+            (~same).sum(), (~same & (marg != 0)).sum())
+        res["sum"] = hold_to_bound(ag[:, 0], ref["aggrs_info"][:, 0, rows], ref["bound_sum"][:, rows], "softmax_sum", live)
+    else:
+        assert np.array_equal(ag, ref["aggrs_info"][:, :, rows], equal_nan=True), "hard-mode aggrs_info not bit-exact"
+    return res
+
+
+def pooled_bound(ref_sc, bound):
+    """2x2 mean pooling of the oracle's soft_colors in the order of the forward's anti-aliasing epilogue and avg_pool2d
+    (window row-major, sum / 4), and the bound on the pooled kernel output: each input anywhere in [ref - bound,
+    ref + bound] (ends rounded outwards to float), the same float adds evaluated on the ends.  -> (pooled, bound)."""
+    def pool(s):
+        return (((s[:, :, 0::2, 0::2] + s[:, :, 0::2, 1::2]) + s[:, :, 1::2, 0::2]) + s[:, :, 1::2, 1::2]) / np.float32(4)
+    r64 = ref_sc.astype(np.float64)
+    with np.errstate(invalid="ignore", over="ignore"):
+        lo64, hi64 = r64 - bound, r64 + bound
+        lo, hi = lo64.astype(np.float32), hi64.astype(np.float32)
+        lo = np.where(lo > lo64, np.nextafter(lo, np.float32(-np.inf)), lo)
+        hi = np.where(hi < hi64, np.nextafter(hi, np.float32(np.inf)), hi)
+        lo, hi = np.where(bound == 0, ref_sc, lo), np.where(bound == 0, ref_sc, hi)
+        p, plo, phi = pool(ref_sc), pool(lo), pool(hi)
+        b = np.maximum(phi.astype(np.float64) - p, p.astype(np.float64) - plo)
+    b = np.where(np.isnan(b), np.inf, b)
+    b[(plo == p) & (phi == p)] = 0.0
+    return p, b
+
+
 def sorted_ids(ids):
     """[B,K,H,W] -> per-pixel ascending id sets with -1 (empty) moved last."""
     a = ids.astype(np.int64).copy()
