@@ -328,6 +328,59 @@ B200R_API int b200r_normal_mapped_lighting_backward(const float* vertices, const
                                                     float directional_intensity, const float* directional_color,
                                                     const float* direction, int with_specular, void* stream);
 
+/* ---- normal and depth G-buffers (Lighting(Gbuffer='normal' | 'depth')) ----------------------------------------------
+ * jrender/renderer/lighting/lighting.py:180-204 with directional_lighting.py:136-144: the textures become ones and the
+ * light terms are replaced, out = clamp(1 * value + 1 * (specular * 0), 0, 1), value = N * 0.5 + 0.5 (mode 0, normal) or
+ * z / M in all three channels (mode 1, depth), z the camera depth of the face centroid and M the max of z over every
+ * (batch, face), NaN if any z is.  specular is the Cook-Torrance term of b200r_surface_lighting_* (0 without that
+ * branch): multiplied by 0, it only matters where it is not finite.
+ * b200r_gbuffer_lighting_*: the flat branch.  Same vertices / faces / metallic / roughness / eye / batch / T / Tm rules
+ * and light parameters as b200r_surface_lighting_* (no ambient: it does not reach the result), out_textures [B, nf, T, 3]
+ * (T = texture_res^2, or ts^3 for n3mr).  Depth also needs camera_eye [camera_eye_batch, 3] (1 or B), the camera
+ * (camera_mode B200R_CAM_*, camera_at_or_direction and camera_up: HOST pointers to 3 floats, as b200r_project_faces_*),
+ * a device workspace of b200r_gbuffer_workspace_floats(B, nf) floats (else B200R_EWORKSPACE) and a device float
+ * depth_max; normal mode ignores all four.  Forward: one launch (normal) or two (depth); the depth workspace then holds
+ * each face's z, which the backward takes as face_depth together with depth_max.  Backward: grad_vertices
+ * [vertices_batch, nv, 3] and grad_metallic / grad_roughness [B, nf, Tm] (each NULL: not needed); two launches for depth
+ * (a workspace of its own, same size), one for normal.  The max's gradient goes in full to every face whose z equals
+ * M.  Material gradients are 0, or NaN where a partial of the specular term is not finite.  No host synchronisation.
+ * b200r_normal_mapped_gbuffer_*: the normal-map branch, mode normal only, N = normalize(n_t . TBN) per texel;
+ * normal_textures [normal_batch, nf, T, 3], tbn [tbn_batch, nf, 3, 3], metallic / roughness [B, nf, T] per texel,
+ * backward writes grad_normal_textures (summed over the batch when normal_batch is 1), grad_vertices (through the
+ * specular term only) and the per-texel material gradients, each NULL: not needed. */
+B200R_API size_t b200r_gbuffer_workspace_floats(int batch_size, int num_faces);
+B200R_API int b200r_gbuffer_lighting_forward(const float* vertices, const int32_t* faces, const float* metallic,
+                                             const float* roughness, const float* eye, const float* camera_eye,
+                                             float* out_textures, float* workspace, size_t workspace_floats, float* depth_max,
+                                             int mode, int B, int vertices_batch, int faces_batch, int eye_batch,
+                                             int camera_eye_batch, int nv, int nf, int T, int Tm, float directional_intensity,
+                                             const float* directional_color, const float* direction, int with_specular,
+                                             const float* camera_at_or_direction, const float* camera_up, int camera_mode,
+                                             void* stream);
+B200R_API int b200r_gbuffer_lighting_backward(const float* vertices, const int32_t* faces, const float* metallic,
+                                              const float* roughness, const float* eye, const float* camera_eye,
+                                              const float* grad_out, const float* face_depth, const float* depth_max,
+                                              float* workspace, size_t workspace_floats, float* grad_vertices,
+                                              float* grad_metallic, float* grad_roughness, int mode, int B, int vertices_batch,
+                                              int faces_batch, int eye_batch, int camera_eye_batch, int nv, int nf, int T,
+                                              int Tm, float directional_intensity, const float* directional_color,
+                                              const float* direction, int with_specular, const float* camera_at_or_direction,
+                                              const float* camera_up, int camera_mode, void* stream);
+B200R_API int b200r_normal_mapped_gbuffer_forward(const float* vertices, const int32_t* faces, const float* normal_textures,
+                                                  const float* tbn, const float* metallic, const float* roughness,
+                                                  const float* eye, float* out_textures, int B, int vertices_batch,
+                                                  int faces_batch, int eye_batch, int normal_batch, int tbn_batch, int nv,
+                                                  int nf, int T, float directional_intensity, const float* directional_color,
+                                                  const float* direction, int with_specular, void* stream);
+B200R_API int b200r_normal_mapped_gbuffer_backward(const float* vertices, const int32_t* faces, const float* normal_textures,
+                                                   const float* tbn, const float* metallic, const float* roughness,
+                                                   const float* eye, const float* grad_out, float* grad_normal_textures,
+                                                   float* grad_vertices, float* grad_metallic, float* grad_roughness, int B,
+                                                   int vertices_batch, int faces_batch, int eye_batch, int normal_batch,
+                                                   int tbn_batch, int nv, int nf, int T, float directional_intensity,
+                                                   const float* directional_color, const float* direction, int with_specular,
+                                                   void* stream);
+
 /* ---- NeRF volume rendering (jrender_vol) -------------------------------------------------------------------------
  * One warp per ray; no atomics, no host synchronisation, no workspace.  Every ray holds at most B200R_VOL_MAX_SAMPLES
  * samples (S for compositing, S + Ni for resampling); beyond that the calls return B200R_EUNSUPPORTED.  num_rays 0 is a

@@ -8,7 +8,10 @@ including the Cook-Torrance specular branch the reference takes by default
 per texel from surface_ResNormals) take the surface branch's normal-map path: one fused kernel forward and one backward
 (b200r_normal_mapped_lighting_*), or the op-by-op directional_lighting_texels.  Meshes with with_SSS and SoftRas
 surface textures take the texture-space subsurface scattering of lighting.py:86-156 (SSS below) on both surface
-branches.  The Gbuffer debug modes are not mirrored.
+branches.  Gbuffer='normal' / 'depth' (directional_lighting.py:136-144) replace the lit colour by the normal map
+(N * 0.5 + 0.5) or the camera depth over its maximum; the surface branches run as fused kernels
+(b200r_gbuffer_lighting_*, b200r_normal_mapped_gbuffer_*, csrc/gbuffer_api.cu), everything else op by op
+(gbuffer_terms below).
 """
 import ctypes as C
 import math
@@ -153,6 +156,134 @@ def directional_lighting_texels(diffuseLight, specularLight, normals, light_inte
     else:
         diffuseLight = diffuseLight + light_intensity * (light_color[:, None, None, :] * cosine[..., None])
     return [diffuseLight, specularLight]
+
+
+GBUFFER_MODES = ('normal', 'depth')
+
+
+class _TiedMax(torch.autograd.Function):
+    """max over every element of x, NaN if any is NaN (numpy's max, as the reference's jt.max is read here).  The
+    gradient goes in full to every element equal to the max -- Jittor's reduce-max gradient, the mask x == max -- not
+    split over ties as torch.max's is."""
+
+    @staticmethod
+    def forward(ctx, x):
+        m = x.max()
+        ctx.save_for_backward(x, m)
+        return m
+
+    @staticmethod
+    def backward(ctx, g):
+        x, m = ctx.saved_tensors
+        return g * (x == m).to(g.dtype)
+
+
+def camera_z(transform, positions):
+    """The z row of transform.tranpos(positions) (transform.py:109-111): the camera-space depth of each position,
+    computed without the perspective division, so that x / z never enters the graph (a position at z = 0 would put
+    0 * inf into the gradient).  positions must be 3-D, under every camera mode (look_at.py:6-7's ValueError)."""
+    if transform is None:
+        raise ValueError("Lighting: Gbuffer='depth' needs the renderer's transform (Lighting(..., transform=...))")
+    if positions.dim() != 3:
+        raise ValueError('vertices Tensor should have 3 dimensions')
+    from .transform import _normalize
+    tr = transform.transformer
+    d, dt = positions.device, positions.dtype
+    if transform.camera_mode == 'projection':
+        return (torch.matmul(positions, tr.R.to(d, dt).transpose(1, 2)[0]) + tr.t.to(d, dt))[..., 2]   # projection.py:19-20
+    eye = tr._eye
+    eye = _t(list(eye) if isinstance(eye, tuple) else eye, positions).to(dt)
+    eye = eye.reshape(-1, 3)
+    if transform.camera_mode == 'look_at':   # look_at.py:26: the z axis, rotation row 3
+        z_axis = _normalize(_t([0, 0, 0], positions).to(dt)[None] - eye)
+    else:
+        z_axis = _normalize(_t(tr.camera_direction, positions).to(dt), dim=0)[None]   # look.py:23
+    return torch.sum((positions - eye[:, None, :]) * z_axis[:, None, :], dim=2)
+
+
+def gbuffer_terms(diffuseLight, specularLight, normals, positions, Gbuffer, transform):
+    """directional_lighting.py:136-144, after the light terms: 'normal' -> (normals * 0.5 + 0.5, specular * 0), 'depth'
+    -> (z / max(z) in all three channels, specular * 0), the max over every batch element and position.  Other values
+    return the terms unchanged."""
+    if Gbuffer == 'normal':
+        return [normals * 0.5 + 0.5, specularLight * 0.0]
+    if Gbuffer == 'depth':
+        z = camera_z(transform, positions)
+        depth = (z / _TiedMax.apply(z))[..., None]
+        return [depth.expand(depth.shape[:-1] + (3,)), specularLight * 0.0]
+    return [diffuseLight, specularLight]
+
+
+class _FusedGbuffer(torch.autograd.Function):
+    """The G-buffer of the flat surface branch, clamp(1 * value + 1 * (specular * 0), 0, 1) over T texels of 4-D or
+    6-D textures: b200r_gbuffer_lighting_*.  Differentiable w.r.t. the vertices and the metallic / roughness textures
+    (through specular * 0); the textures (all ones in this mode) get no gradient."""
+
+    @staticmethod
+    def forward(ctx, vertices, metallic, roughness, faces, eye, cam_eye, shape, params, cam):
+        v = vertices.contiguous()
+        B, nf = shape[0], shape[1]
+        T = int(torch.Size(shape[2:]).numel()) // 3
+        Tm = 0 if metallic is None else metallic[0, 0].numel()
+        dev = v.device
+        out = torch.empty(shape, dtype=torch.float32, device=dev)
+        mode, dir_i, dir_c, direction, with_spec = params
+        depth = mode == GBUFFER_MODES.index('depth')
+        nws = _lib.lib().b200r_gbuffer_workspace_floats(B, nf) if depth else 0
+        ws = torch.empty((nws,), dtype=torch.float32, device=dev) if depth else None
+        dmax = torch.empty((1,), dtype=torch.float32, device=dev) if depth else None
+        at, up, cmode = cam if depth else ((0.0, 0.0, 0.0), (0.0, 1.0, 0.0), 0)
+        args = (mode, B, v.shape[0], faces.shape[0], 0 if eye is None else eye.shape[0],
+                0 if cam_eye is None else cam_eye.shape[0], v.shape[1], nf, T, Tm, float(dir_i), _f3(dir_c),
+                _f3(direction), int(bool(with_spec)), _f3(at), _f3(up), int(cmode))
+        _lib.call("b200r_gbuffer_lighting_forward", dev, v, faces, metallic, roughness, eye, cam_eye, out, ws, nws, dmax,
+                  *args)
+        ctx.save_for_backward(v, faces, metallic, roughness, eye, cam_eye, ws, dmax)
+        ctx.args, ctx.nws = args, nws
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        v, faces, metallic, roughness, eye, cam_eye, face_z, dmax = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        gv = torch.empty_like(v) if need[0] else None
+        gm = torch.empty_like(metallic) if need[1] else None
+        gr = torch.empty_like(roughness) if need[2] else None
+        ws = torch.empty((ctx.nws,), dtype=torch.float32, device=v.device) if ctx.nws else None
+        _lib.call("b200r_gbuffer_lighting_backward", v.device, v, faces, metallic, roughness, eye, cam_eye,
+                  grad_out.contiguous(), face_z, dmax, ws, ctx.nws, gv, gm, gr, *ctx.args)
+        return gv, gm, gr, None, None, None, None, None, None
+
+
+class _FusedNormalMappedGbuffer(torch.autograd.Function):
+    """The normal G-buffer of the normal-map branch, clamp(1 * (N_t * 0.5 + 0.5) + 1 * (specular * 0), 0, 1) with
+    N_t = normalize(n_t . TBN) per texel: b200r_normal_mapped_gbuffer_*.  Differentiable w.r.t. the normal textures,
+    and, through specular * 0, the vertices and the per-texel metallic / roughness; not w.r.t. the TBN."""
+
+    @staticmethod
+    def forward(ctx, vertices, normal_textures, metallic, roughness, faces, tbn, eye, params):
+        v, nt = vertices.contiguous(), normal_textures.contiguous()
+        B, nf, T = params[0]
+        dir_i, dir_c, direction, with_spec = params[1:]
+        out = torch.empty((B, nf, T, 3), dtype=torch.float32, device=v.device)
+        args = (B, v.shape[0], faces.shape[0], 0 if eye is None else eye.shape[0], nt.shape[0], tbn.shape[0], v.shape[1],
+                nf, T, float(dir_i), _f3(dir_c), _f3(direction), int(bool(with_spec)))
+        _lib.call("b200r_normal_mapped_gbuffer_forward", v.device, v, faces, nt, tbn, metallic, roughness, eye, out, *args)
+        ctx.save_for_backward(v, nt, metallic, roughness, faces, tbn, eye)
+        ctx.args = args
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        v, nt, metallic, roughness, faces, tbn, eye = ctx.saved_tensors
+        need = ctx.needs_input_grad
+        gv = torch.empty_like(v) if need[0] else None
+        gn = torch.empty_like(nt) if need[1] else None
+        gm = torch.empty_like(metallic) if need[2] else None
+        gr = torch.empty_like(roughness) if need[3] else None
+        _lib.call("b200r_normal_mapped_gbuffer_backward", v.device, v, faces, nt, tbn, metallic, roughness, eye,
+                  grad_out.contiguous(), gn, gv, gm, gr, *ctx.args)
+        return gv, gn, gm, gr, None, None, None, None
 
 
 class _FusedNormalMappedLighting(torch.autograd.Function):
@@ -426,17 +557,21 @@ class AmbientLighting(nn.Module):
 
 
 class DirectionalLighting(nn.Module):
-    def __init__(self, light_intensity=0.5, light_color=(1, 1, 1), light_direction=(0, 1, 0)):
+    def __init__(self, light_intensity=0.5, light_color=(1, 1, 1), light_direction=(0, 1, 0), Gbuffer='None',
+                 transform=None):
         super(DirectionalLighting, self).__init__()
         self.light_intensity = light_intensity
         self.light_color = light_color
         self.light_direction = light_direction
+        self.Gbuffer = Gbuffer
+        self.transform = transform
 
     def forward(self, diffuseLight, specularLight, normals, positions=None, eye=None, with_specular=False,
                 metallic_textures=None, roughness_textures=None):
-        return directional_lighting(diffuseLight, specularLight, normals, self.light_intensity, self.light_color,
-                                    self.light_direction, positions, eye, with_specular, metallic_textures,
-                                    roughness_textures)
+        diffuseLight, specularLight = directional_lighting(
+            diffuseLight, specularLight, normals, self.light_intensity, self.light_color, self.light_direction,
+            positions, eye, with_specular, metallic_textures, roughness_textures)
+        return gbuffer_terms(diffuseLight, specularLight, normals, positions, self.Gbuffer, self.transform)
 
     execute = forward
 
@@ -451,13 +586,15 @@ class Lighting(nn.Module):
         super(Lighting, self).__init__()
         if light_mode not in ['surface', 'vertex']:
             raise ValueError('Lighting mode only support surface and vertex')
-        if Gbuffer not in ('None', None, 'albedo'):
-            raise NotImplementedError("Gbuffer=%r (render2 debug outputs) is outside this repo's scope" % (Gbuffer,))
+        # The reference lights normally for any other string; a typo raising here is deliberate.
+        if Gbuffer not in ('None', None, 'albedo') + GBUFFER_MODES:
+            raise ValueError("Gbuffer must be 'None', 'albedo', 'normal' or 'depth', got %r" % (Gbuffer,))
         self.Gbuffer = Gbuffer
         self.transform = transform
         self.light_mode = light_mode
         self.ambient = AmbientLighting(intensity_ambient, color_ambient)
-        self.directionals = nn.ModuleList([DirectionalLighting(intensity_directionals, color_directionals, directions)])
+        self.directionals = nn.ModuleList([DirectionalLighting(intensity_directionals, color_directionals, directions,
+                                                               Gbuffer, transform)])
 
     fused = True   # CUDA float32 surface-mode inputs take the one-launch kernel (b200r_surface_lighting_forward)
     sss_grad = False   # with_SSS meshes: differentiate SSS (SSS(..., grad=True)); off, its result carries no graph
@@ -581,9 +718,149 @@ class Lighting(nn.Module):
         mesh.textures = torch.clamp(SSS(diffuseLight, specularLight, mesh, grad=self.sss_grad), 0.0, 1.0)
         return mesh
 
+    def _light_params(self, mesh, eyes, spec_ok):
+        """(eye [1|B, 3] or None, with_specular, directional intensity, colour, host-normalised direction) for the
+        G-buffer kernels; None where the eye batch does not fit."""
+        d = self.directionals[0]
+        spec = bool(mesh.with_specular) and eyes is not None and spec_ok
+        eye = None
+        if spec:
+            eye = _t(eyes, mesh.vertices).reshape(-1, 3).contiguous()
+            if eye.shape[0] not in (1, mesh.textures.shape[0]):
+                return None
+        return eye, spec, d.light_intensity, d.light_color, _normalized_direction(d.light_direction)
+
+    def _fused_gbuffer(self, mesh, eyes):
+        """The flat surface branch's G-buffer in one launch (normal) or two (depth), or None where it runs op by op:
+        anything _fusable rejects, and for depth a camera other than look_at / look or an eye that requires grad
+        (Transform._fused_projector's rule)."""
+        if not self._fusable(mesh, eyes):
+            return None
+        v, tx = mesh.vertices, mesh.textures
+        B = tx.shape[0]
+        mode = GBUFFER_MODES.index(self.Gbuffer)
+        cam_eye, cam = None, None
+        if self.Gbuffer == 'depth':
+            tr = self.transform
+            if tr is None or tr._fused_projector(mesh) is None:
+                return None
+            from .preraster import CAM_MODES
+            t = tr.transformer
+            e = t._eye
+            cam_eye = (e.detach().to(v.device, torch.float32) if isinstance(e, torch.Tensor)
+                       else _t(list(e) if isinstance(e, tuple) else e, v)).reshape(-1, 3).contiguous()
+            if cam_eye.shape[0] not in (1, B) or v.shape[0] not in (1, B) or mesh.faces.shape[0] not in (1, B):
+                return None
+            if tr.camera_mode == 'look_at':
+                cam = ((0.0, 0.0, 0.0), (0.0, 1.0, 0.0), CAM_MODES['look_at'])
+            elif t.coordinate in ('right', 'left'):
+                cam = (t.camera_direction, t.up, CAM_MODES['look_' + t.coordinate])
+            else:
+                return None
+        lp = self._light_params(mesh, eyes, mesh.metallic_textures is not None and mesh.roughness_textures is not None)
+        if lp is None:
+            return None
+        eye, spec, dir_i, dir_c, direction = lp
+        faces = mesh.faces if mesh.faces.dtype == torch.int32 else mesh.faces.int()
+        return _FusedGbuffer.apply(v, mesh.metallic_textures.contiguous() if spec else None,
+                                   mesh.roughness_textures.contiguous() if spec else None, faces.contiguous(), eye,
+                                   cam_eye, tuple(tx.shape), (mode, dir_i, dir_c, direction, spec), cam)
+
+    def _fused_normal_mapped_gbuffer(self, mesh, eyes):
+        """The normal-map branch's normal G-buffer in one launch, or None under _fused_normal_mapped's rules."""
+        if not self._fusable(mesh, eyes):
+            return None
+        v, tx, nt, tbn = mesh.vertices, mesh.textures, mesh.normal_textures, mesh.TBN
+        B, nf, T = tx.shape[:3]
+        for x in (nt, tbn):
+            if x.dtype != torch.float32 or x.device != v.device or x.shape[0] not in (1, B):
+                return None
+        if tbn.requires_grad:
+            return None
+        lp = self._light_params(mesh, eyes, mesh.metallic_textures is not None and mesh.roughness_textures is not None)
+        if lp is None:
+            return None
+        eye, spec, dir_i, dir_c, direction = lp
+        met = rou = None
+        if spec:
+            if mesh.metallic_textures.shape[2] not in (1, T) or mesh.roughness_textures.shape[2] not in (1, T):
+                return None
+            met = mesh.metallic_textures.expand(B, nf, T, 1).contiguous()
+            rou = mesh.roughness_textures.expand(B, nf, T, 1).contiguous()
+        faces = mesh.faces if mesh.faces.dtype == torch.int32 else mesh.faces.int()
+        # without the specular branch the vertices do not reach the result (the mirror's graph has no path to them)
+        return _FusedNormalMappedGbuffer.apply(v if spec else v.detach(), nt, met, rou, faces.contiguous(), tbn.contiguous(), eye,
+                                               ((B, nf, T), dir_i, dir_c, direction, spec))
+
+    def _gbuffer(self, mesh, eyes):
+        """Gbuffer='normal' / 'depth': lighting.py:180-220 with directional_lighting.py:136-144.  The textures become
+        ones (the caller's get no gradient), the light terms are replaced, and the usual composition follows: the clamp,
+        or SSS for with_SSS meshes."""
+        if self.light_mode == 'surface' and not (mesh.with_SSS and mesh.textures.dim() == 4):
+            if mesh.normal_textures is not None:
+                self._check_normal_map(mesh)
+                if self.Gbuffer == 'depth':   # positions unsqueezed to 4-D reach look_at's check
+                    raise ValueError('vertices Tensor should have 3 dimensions')
+                lit = self._fused_normal_mapped_gbuffer(mesh, eyes)
+            else:
+                lit = self._fused_gbuffer(mesh, eyes)
+            if lit is not None:
+                mesh.textures = lit
+                return mesh
+        mesh.textures = torch.ones_like(mesh.textures)
+        if self.light_mode == 'surface':
+            if mesh.normal_textures is not None:
+                self._check_normal_map(mesh)
+                positions = torch.sum(mesh.face_vertices, dim=2) / 3.0
+                diffuseLight = torch.zeros(mesh.textures.shape, dtype=mesh.textures.dtype, device=mesh.vertices.device)
+                specularLight = torch.zeros_like(diffuseLight)
+                diffuseLight = self.ambient(diffuseLight)
+                normals = mesh.surface_ResNormals
+                for d in self.directionals:
+                    diffuseLight, specularLight = directional_lighting_texels(
+                        diffuseLight, specularLight, normals, d.light_intensity, d.light_color, d.light_direction,
+                        positions, eyes, mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
+                    diffuseLight, specularLight = gbuffer_terms(diffuseLight, specularLight, normals,
+                                                                positions.unsqueeze(2), d.Gbuffer, d.transform)
+            else:
+                diffuseLight = torch.zeros(mesh.faces.shape, dtype=torch.float32, device=mesh.vertices.device)
+                specularLight = torch.zeros_like(diffuseLight)
+                diffuseLight = self.ambient(diffuseLight)
+                for directional in self.directionals:
+                    diffuseLight, specularLight = directional(
+                        diffuseLight, specularLight, mesh.surface_normals, torch.sum(mesh.face_vertices, dim=2) / 3.0,
+                        eyes, mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
+                diffuseLight = diffuseLight[:, :, None, :]
+                specularLight = specularLight[:, :, None, :]
+            if mesh.with_SSS and mesh.textures.dim() == 4:
+                mesh.textures = torch.clamp(SSS(diffuseLight, specularLight, mesh, grad=self.sss_grad), 0.0, 1.0)
+            elif mesh.textures.dim() == 4:
+                mesh.textures = torch.clamp(mesh.textures * diffuseLight + torch.ones_like(mesh.textures) * specularLight,
+                                            0.0, 1.0)
+            elif mesh.textures.dim() == 6:
+                mesh.textures = torch.clamp(mesh.textures * diffuseLight[:, :, :, None, None, :] +
+                                            torch.ones_like(mesh.textures) * specularLight[:, :, :, None, None, :], 0.0, 1.0)
+        elif self.light_mode == 'vertex':
+            diffuseLight = torch.zeros(mesh.vertices.shape, dtype=torch.float32, device=mesh.vertices.device)
+            specularLight = torch.zeros_like(diffuseLight)
+            diffuseLight = self.ambient(diffuseLight)
+            for directional in self.directionals:
+                diffuseLight, specularLight = directional(
+                    diffuseLight, specularLight, mesh.vertex_normals, mesh.vertices, eyes,
+                    mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
+            if mesh.textures.dim() == 4:
+                mesh.textures = torch.clamp(mesh.textures * diffuseLight[:, :, None, :] +
+                                            torch.ones_like(mesh.textures) * specularLight[:, :, None, :], 0.0, 1.0)
+            elif mesh.textures.dim() == 6:
+                mesh.textures = torch.clamp(mesh.textures * diffuseLight[:, :, None, None, None, :] +
+                                            torch.ones_like(mesh.textures) * specularLight[:, :, None, None, None, :], 0.0, 1.0)
+        return mesh
+
     def forward(self, mesh, eyes=None):
         if self.Gbuffer == "albedo":
             return mesh
+        if self.Gbuffer in GBUFFER_MODES:
+            return self._gbuffer(mesh, eyes)
         if self.light_mode == 'surface' and mesh.with_SSS and mesh.textures.dim() == 4:
             return self._subsurface(mesh, eyes)
         if self.light_mode == 'surface' and mesh.normal_textures is not None:
