@@ -505,7 +505,6 @@ def SSS(diffuseLight, specular, mesh, grad=False):
 
     The batch must be 1, the mesh must carry face_texcoords, and its textures must hold texture_res^2 texels per face
     (ValueError otherwise)."""
-    from . import io
     tx = mesh.textures
     if tx.dim() != 4 or tx.shape[0] != 1:
         raise ValueError("SSS: needs a batch of one mesh with SoftRas surface textures [1, nf, T, 3], got %s"
@@ -518,30 +517,15 @@ def SSS(diffuseLight, specular, mesh, grad=False):
         raise ValueError("SSS: %d texels per face, texture_res %d needs %d" % (T, R, R * R))
     if tuple(ftc.shape) != (1, nf, 3, 2):
         raise ValueError("SSS: face_texcoords %s do not match %d faces" % (tuple(ftc.shape), nf))
-    dev = tx.device
-    S = SSS_IMAGE_SIZE
-    if grad and torch.is_grad_enabled():
-        if ftc.requires_grad:
-            raise ValueError("SSS: face_texcoords require grad, but no gradient flows to them")
-        if any(t.requires_grad for t in (diffuseLight, specular, tx, mesh.face_vertices)):
-            world_map, irradiance_map, specular_map = _sss_maps(diffuseLight, specular, mesh)
-            stretch_u, stretch_v = _SSSStretch.apply(world_map)
-            final_map = _SSSPyramid.apply(stretch_u, stretch_v, irradiance_map, specular_map)
-            return _SSSBake.apply(final_map, ftc[0].to(dev, torch.float32).contiguous(), R)[None]
-    with torch.no_grad():
+    track = grad and torch.is_grad_enabled()
+    if track and ftc.requires_grad:
+        raise ValueError("SSS: face_texcoords require grad, but no gradient flows to them")
+    track = track and any(t.requires_grad for t in (diffuseLight, specular, tx, mesh.face_vertices))
+    with torch.set_grad_enabled(track):
         world_map, irradiance_map, specular_map = _sss_maps(diffuseLight, specular, mesh)
-        stretch_u = torch.empty((S, S), dtype=torch.float32, device=dev)
-        stretch_v = torch.empty_like(stretch_u)
-        _lib.call("b200r_sss_stretch", dev, world_map, stretch_u, stretch_v, S, S)
-        taps, widths, weights, L = _sss_levels()
-        nbytes = _lib.lib().b200r_sss_workspace_bytes(S, S)
-        workspace = torch.empty((nbytes,), dtype=torch.uint8, device=dev)
-        final_map = torch.empty((S, S, 3), dtype=torch.float32, device=dev)
-        _lib.call("b200r_sss_blur_pyramid", dev, stretch_u, stretch_v, irradiance_map, specular_map, final_map, workspace,
-                  nbytes, taps, widths, weights, L, S, S)
-        final = io.bake_textures_for_softras(final_map, ftc[0], torch.ones((nf, R * R, 3), dtype=torch.float32, device=dev),
-                                             torch.ones((nf,), dtype=torch.int32, device=dev), device=dev)
-    return final[None]
+        stretch_u, stretch_v = _SSSStretch.apply(world_map)
+        final_map = _SSSPyramid.apply(stretch_u, stretch_v, irradiance_map, specular_map)
+        return _SSSBake.apply(final_map, ftc[0].to(tx.device, torch.float32).contiguous(), R)[None]
 
 
 class AmbientLighting(nn.Module):
@@ -620,22 +604,6 @@ class Lighting(nn.Module):
             return False
         return True
 
-    def _fused_surface(self, mesh, eyes):
-        v = mesh.vertices
-        d = self.directionals[0]
-        eye = None
-        spec = bool(mesh.with_specular) and eyes is not None and mesh.metallic_textures is not None and mesh.roughness_textures is not None
-        if spec:
-            eye = _t(eyes, v).reshape(-1, 3).contiguous()
-            if eye.shape[0] not in (1, mesh.textures.shape[0]):
-                return None
-        faces = mesh.faces if mesh.faces.dtype == torch.int32 else mesh.faces.int()
-        params = (self.ambient.light_intensity, self.ambient.light_color, d.light_intensity, d.light_color,
-                  _normalized_direction(d.light_direction), spec)
-        return _FusedSurfaceLighting.apply(v, mesh.textures, faces.contiguous(),
-                                           mesh.metallic_textures.contiguous() if spec else None,
-                                           mesh.roughness_textures.contiguous() if spec else None, eye, params)
-
     def _check_normal_map(self, mesh):
         tx, nt, tbn = mesh.textures, mesh.normal_textures, mesh.TBN
         if tx.dim() != 4:
@@ -646,99 +614,26 @@ class Lighting(nn.Module):
             raise ValueError("Lighting: normal_textures %s / TBN %s do not match textures %s"
                              % (tuple(nt.shape), None if tbn is None else tuple(tbn.shape), tuple(tx.shape)))
 
-    def _fused_normal_mapped(self, mesh, eyes):
-        """The normal-map branch in one launch, or None where it must run op by op: anything _fusable rejects, an eye or
-        TBN that requires grad, or tensors the kernel does not take (dtype, device, batch, material texel count)."""
+    def _fused(self, mesh, eyes):
+        """The surface branch in one fused kernel: lit or G-buffer, with face normals or a normal map's texel normals
+        (_FusedSurfaceLighting, _FusedNormalMappedLighting, _FusedGbuffer, _FusedNormalMappedGbuffer).  None where it
+        runs op by op: anything _fusable rejects; a normal map or TBN of another dtype, device or batch, a TBN that
+        requires grad, or metallic / roughness with other than 1 or T texels per face; an eye batch other than 1 or B;
+        and for depth a camera other than look_at / look or an eye that requires grad (Transform._fused_projector's
+        rule)."""
+        normal_map = mesh.normal_textures is not None
+        if normal_map and self.Gbuffer == 'depth':   # positions unsqueezed to 4-D reach look_at's check
+            raise ValueError('vertices Tensor should have 3 dimensions')
         if not self._fusable(mesh, eyes):
             return None
         v, tx, nt, tbn = mesh.vertices, mesh.textures, mesh.normal_textures, mesh.TBN
-        B, nf, T = tx.shape[:3]
-        for x in (nt, tbn):
-            if x.dtype != torch.float32 or x.device != v.device or x.shape[0] not in (1, B):
+        B, nf = tx.shape[:2]
+        if normal_map:
+            for x in (nt, tbn):
+                if x.dtype != torch.float32 or x.device != v.device or x.shape[0] not in (1, B):
+                    return None
+            if tbn.requires_grad:
                 return None
-        if tbn.requires_grad:
-            return None
-        d = self.directionals[0]
-        spec = bool(mesh.with_specular) and eyes is not None and mesh.metallic_textures is not None \
-            and mesh.roughness_textures is not None
-        eye = met = rou = None
-        if spec:
-            eye = _t(eyes, v).reshape(-1, 3).contiguous()
-            if eye.shape[0] not in (1, B):
-                return None
-            if mesh.metallic_textures.shape[2] not in (1, T) or mesh.roughness_textures.shape[2] not in (1, T):
-                return None
-            met = mesh.metallic_textures.expand(B, nf, T, 1).contiguous()   # a per-face value broadcasts over the texels
-            rou = mesh.roughness_textures.expand(B, nf, T, 1).contiguous()
-        faces = mesh.faces if mesh.faces.dtype == torch.int32 else mesh.faces.int()
-        params = (self.ambient.light_intensity, self.ambient.light_color, d.light_intensity, d.light_color,
-                  _normalized_direction(d.light_direction), spec)
-        return _FusedNormalMappedLighting.apply(v, tx, nt, met, rou, faces.contiguous(), tbn.contiguous(), eye, params)
-
-    def _normal_mapped(self, mesh, eyes):
-        """lighting.py:186-192 and 200-201: the surface branch with mesh.normal_textures."""
-        self._check_normal_map(mesh)
-        lit = self._fused_normal_mapped(mesh, eyes)
-        if lit is None:
-            diffuseLight = torch.zeros(mesh.textures.shape, dtype=mesh.textures.dtype, device=mesh.vertices.device)
-            specularLight = torch.zeros_like(diffuseLight)
-            diffuseLight = self.ambient(diffuseLight)
-            for d in self.directionals:
-                diffuseLight, specularLight = directional_lighting_texels(
-                    diffuseLight, specularLight, mesh.surface_ResNormals, d.light_intensity, d.light_color,
-                    d.light_direction, torch.sum(mesh.face_vertices, dim=2) / 3.0, eyes, mesh.with_specular,
-                    mesh.metallic_textures, mesh.roughness_textures)
-            lit = torch.clamp(mesh.textures * diffuseLight + torch.ones_like(mesh.textures) * specularLight, 0.0, 1.0)
-        mesh.textures = lit
-        return mesh
-
-    def _subsurface(self, mesh, eyes):
-        """lighting.py:182-201 with mesh.with_SSS and 4-D textures: the op-by-op diffuse and specular light of either
-        surface branch (per face, or per texel with a normal map), then clamp(SSS(diffuse, specular, mesh), 0, 1)."""
-        if mesh.normal_textures is not None:
-            self._check_normal_map(mesh)
-            diffuseLight = torch.zeros(mesh.textures.shape, dtype=mesh.textures.dtype, device=mesh.vertices.device)
-            specularLight = torch.zeros_like(diffuseLight)
-            diffuseLight = self.ambient(diffuseLight)
-            for d in self.directionals:
-                diffuseLight, specularLight = directional_lighting_texels(
-                    diffuseLight, specularLight, mesh.surface_ResNormals, d.light_intensity, d.light_color,
-                    d.light_direction, torch.sum(mesh.face_vertices, dim=2) / 3.0, eyes, mesh.with_specular,
-                    mesh.metallic_textures, mesh.roughness_textures)
-        else:
-            diffuseLight = torch.zeros(mesh.faces.shape, dtype=torch.float32, device=mesh.vertices.device)
-            specularLight = torch.zeros_like(diffuseLight)
-            diffuseLight = self.ambient(diffuseLight)
-            for directional in self.directionals:
-                diffuseLight, specularLight = directional(
-                    diffuseLight, specularLight, mesh.surface_normals, torch.sum(mesh.face_vertices, dim=2) / 3.0, eyes,
-                    mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
-            diffuseLight = diffuseLight[:, :, None, :]
-            specularLight = specularLight[:, :, None, :]
-        mesh.textures = torch.clamp(SSS(diffuseLight, specularLight, mesh, grad=self.sss_grad), 0.0, 1.0)
-        return mesh
-
-    def _light_params(self, mesh, eyes, spec_ok):
-        """(eye [1|B, 3] or None, with_specular, directional intensity, colour, host-normalised direction) for the
-        G-buffer kernels; None where the eye batch does not fit."""
-        d = self.directionals[0]
-        spec = bool(mesh.with_specular) and eyes is not None and spec_ok
-        eye = None
-        if spec:
-            eye = _t(eyes, mesh.vertices).reshape(-1, 3).contiguous()
-            if eye.shape[0] not in (1, mesh.textures.shape[0]):
-                return None
-        return eye, spec, d.light_intensity, d.light_color, _normalized_direction(d.light_direction)
-
-    def _fused_gbuffer(self, mesh, eyes):
-        """The flat surface branch's G-buffer in one launch (normal) or two (depth), or None where it runs op by op:
-        anything _fusable rejects, and for depth a camera other than look_at / look or an eye that requires grad
-        (Transform._fused_projector's rule)."""
-        if not self._fusable(mesh, eyes):
-            return None
-        v, tx = mesh.vertices, mesh.textures
-        B = tx.shape[0]
-        mode = GBUFFER_MODES.index(self.Gbuffer)
         cam_eye, cam = None, None
         if self.Gbuffer == 'depth':
             tr = self.transform
@@ -757,150 +652,118 @@ class Lighting(nn.Module):
                 cam = (t.camera_direction, t.up, CAM_MODES['look_' + t.coordinate])
             else:
                 return None
-        lp = self._light_params(mesh, eyes, mesh.metallic_textures is not None and mesh.roughness_textures is not None)
-        if lp is None:
+        spec = bool(mesh.with_specular) and eyes is not None and mesh.metallic_textures is not None \
+            and mesh.roughness_textures is not None
+        eye = met = rou = None
+        if spec:
+            eye = _t(eyes, v).reshape(-1, 3).contiguous()
+            if eye.shape[0] not in (1, B):
+                return None
+            met, rou = mesh.metallic_textures, mesh.roughness_textures
+            if normal_map:
+                T = tx.shape[2]
+                if met.shape[2] not in (1, T) or rou.shape[2] not in (1, T):
+                    return None
+                met, rou = met.expand(B, nf, T, 1), rou.expand(B, nf, T, 1)   # a per-face value broadcasts over the texels
+            met, rou = met.contiguous(), rou.contiguous()
+        faces = (mesh.faces if mesh.faces.dtype == torch.int32 else mesh.faces.int()).contiguous()
+        d = self.directionals[0]
+        light = (d.light_intensity, d.light_color, _normalized_direction(d.light_direction), spec)
+        if self.Gbuffer in GBUFFER_MODES:
+            if normal_map:
+                # without the specular branch the vertices do not reach the result (the mirror's graph has no path to them)
+                return _FusedNormalMappedGbuffer.apply(v if spec else v.detach(), nt, met, rou, faces, tbn.contiguous(),
+                                                       eye, (tuple(tx.shape[:3]),) + light)
+            return _FusedGbuffer.apply(v, met, rou, faces, eye, cam_eye, tuple(tx.shape),
+                                       (GBUFFER_MODES.index(self.Gbuffer),) + light, cam)
+        light = (self.ambient.light_intensity, self.ambient.light_color) + light
+        if normal_map:
+            return _FusedNormalMappedLighting.apply(v, tx, nt, met, rou, faces, tbn.contiguous(), eye, light)
+        return _FusedSurfaceLighting.apply(v, tx, faces, met, rou, eye, light)
+
+    def _fused_on(self, mesh, eyes, normal_map, gbuffer):
+        """_fused on one kernel's route only, None off it: a caller that asks for one kernel by name learns whether
+        that kernel, and no other, takes these inputs."""
+        if (mesh.normal_textures is not None) != normal_map or (self.Gbuffer in GBUFFER_MODES) != gbuffer:
             return None
-        eye, spec, dir_i, dir_c, direction = lp
-        faces = mesh.faces if mesh.faces.dtype == torch.int32 else mesh.faces.int()
-        return _FusedGbuffer.apply(v, mesh.metallic_textures.contiguous() if spec else None,
-                                   mesh.roughness_textures.contiguous() if spec else None, faces.contiguous(), eye,
-                                   cam_eye, tuple(tx.shape), (mode, dir_i, dir_c, direction, spec), cam)
+        return self._fused(mesh, eyes)
+
+    def _fused_surface(self, mesh, eyes):
+        return self._fused_on(mesh, eyes, normal_map=False, gbuffer=False)
+
+    def _fused_normal_mapped(self, mesh, eyes):
+        return self._fused_on(mesh, eyes, normal_map=True, gbuffer=False)
+
+    def _fused_gbuffer(self, mesh, eyes):
+        return self._fused_on(mesh, eyes, normal_map=False, gbuffer=True)
 
     def _fused_normal_mapped_gbuffer(self, mesh, eyes):
-        """The normal-map branch's normal G-buffer in one launch, or None under _fused_normal_mapped's rules."""
-        if not self._fusable(mesh, eyes):
-            return None
-        v, tx, nt, tbn = mesh.vertices, mesh.textures, mesh.normal_textures, mesh.TBN
-        B, nf, T = tx.shape[:3]
-        for x in (nt, tbn):
-            if x.dtype != torch.float32 or x.device != v.device or x.shape[0] not in (1, B):
-                return None
-        if tbn.requires_grad:
-            return None
-        lp = self._light_params(mesh, eyes, mesh.metallic_textures is not None and mesh.roughness_textures is not None)
-        if lp is None:
-            return None
-        eye, spec, dir_i, dir_c, direction = lp
-        met = rou = None
-        if spec:
-            if mesh.metallic_textures.shape[2] not in (1, T) or mesh.roughness_textures.shape[2] not in (1, T):
-                return None
-            met = mesh.metallic_textures.expand(B, nf, T, 1).contiguous()
-            rou = mesh.roughness_textures.expand(B, nf, T, 1).contiguous()
-        faces = mesh.faces if mesh.faces.dtype == torch.int32 else mesh.faces.int()
-        # without the specular branch the vertices do not reach the result (the mirror's graph has no path to them)
-        return _FusedNormalMappedGbuffer.apply(v if spec else v.detach(), nt, met, rou, faces.contiguous(), tbn.contiguous(), eye,
-                                               ((B, nf, T), dir_i, dir_c, direction, spec))
+        return self._fused_on(mesh, eyes, normal_map=True, gbuffer=True)
 
-    def _gbuffer(self, mesh, eyes):
-        """Gbuffer='normal' / 'depth': lighting.py:180-220 with directional_lighting.py:136-144.  The textures become
-        ones (the caller's get no gradient), the light terms are replaced, and the usual composition follows: the clamp,
-        or SSS for with_SSS meshes."""
-        if self.light_mode == 'surface' and not (mesh.with_SSS and mesh.textures.dim() == 4):
-            if mesh.normal_textures is not None:
-                self._check_normal_map(mesh)
-                if self.Gbuffer == 'depth':   # positions unsqueezed to 4-D reach look_at's check
-                    raise ValueError('vertices Tensor should have 3 dimensions')
-                lit = self._fused_normal_mapped_gbuffer(mesh, eyes)
-            else:
-                lit = self._fused_gbuffer(mesh, eyes)
-            if lit is not None:
-                mesh.textures = lit
-                return mesh
-        mesh.textures = torch.ones_like(mesh.textures)
-        if self.light_mode == 'surface':
-            if mesh.normal_textures is not None:
-                self._check_normal_map(mesh)
-                positions = torch.sum(mesh.face_vertices, dim=2) / 3.0
-                diffuseLight = torch.zeros(mesh.textures.shape, dtype=mesh.textures.dtype, device=mesh.vertices.device)
-                specularLight = torch.zeros_like(diffuseLight)
-                diffuseLight = self.ambient(diffuseLight)
-                normals = mesh.surface_ResNormals
-                for d in self.directionals:
-                    diffuseLight, specularLight = directional_lighting_texels(
-                        diffuseLight, specularLight, normals, d.light_intensity, d.light_color, d.light_direction,
-                        positions, eyes, mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
-                    diffuseLight, specularLight = gbuffer_terms(diffuseLight, specularLight, normals,
-                                                                positions.unsqueeze(2), d.Gbuffer, d.transform)
-            else:
-                diffuseLight = torch.zeros(mesh.faces.shape, dtype=torch.float32, device=mesh.vertices.device)
-                specularLight = torch.zeros_like(diffuseLight)
-                diffuseLight = self.ambient(diffuseLight)
-                for directional in self.directionals:
-                    diffuseLight, specularLight = directional(
-                        diffuseLight, specularLight, mesh.surface_normals, torch.sum(mesh.face_vertices, dim=2) / 3.0,
-                        eyes, mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
-                diffuseLight = diffuseLight[:, :, None, :]
-                specularLight = specularLight[:, :, None, :]
-            if mesh.with_SSS and mesh.textures.dim() == 4:
-                mesh.textures = torch.clamp(SSS(diffuseLight, specularLight, mesh, grad=self.sss_grad), 0.0, 1.0)
-            elif mesh.textures.dim() == 4:
-                mesh.textures = torch.clamp(mesh.textures * diffuseLight + torch.ones_like(mesh.textures) * specularLight,
-                                            0.0, 1.0)
-            elif mesh.textures.dim() == 6:
-                mesh.textures = torch.clamp(mesh.textures * diffuseLight[:, :, :, None, None, :] +
-                                            torch.ones_like(mesh.textures) * specularLight[:, :, :, None, None, :], 0.0, 1.0)
-        elif self.light_mode == 'vertex':
+    def _directional(self, directional, diffuseLight, specularLight, mesh, eyes):
+        """directional_lighting.py:54-145: one directional light's terms, then its G-buffer replacement, at the vertex
+        normals in vertex mode, else at the face centroids with the normal map's texel normals or the face normals."""
+        material = (mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
+        if self.light_mode == 'vertex':
+            return directional(diffuseLight, specularLight, mesh.vertex_normals, mesh.vertices, eyes, *material)
+        # the normals before the centroids: the order autograd sums the vertex gradient's terms in
+        normals = mesh.surface_normals if mesh.normal_textures is None else mesh.surface_ResNormals
+        positions = torch.sum(mesh.face_vertices, dim=2) / 3.0
+        if mesh.normal_textures is None:
+            return directional(diffuseLight, specularLight, normals, positions, eyes, *material)
+        diffuseLight, specularLight = directional_lighting_texels(
+            diffuseLight, specularLight, normals, directional.light_intensity, directional.light_color,
+            directional.light_direction, positions, eyes, *material)
+        return gbuffer_terms(diffuseLight, specularLight, normals, positions.unsqueeze(2), directional.Gbuffer,
+                             directional.transform)
+
+    def _light_terms(self, mesh, eyes):
+        """lighting.py:182-213: (diffuse, specular) from zeros, the ambient light and each directional light, shaped for
+        composition: [B, nv, 3] per vertex in vertex mode, [B, nf, T, 3] per texel with a normal map, else [B, nf, 1, 3]
+        per face."""
+        per_face = self.light_mode == 'surface' and mesh.normal_textures is None
+        if self.light_mode == 'vertex':
             diffuseLight = torch.zeros(mesh.vertices.shape, dtype=torch.float32, device=mesh.vertices.device)
-            specularLight = torch.zeros_like(diffuseLight)
-            diffuseLight = self.ambient(diffuseLight)
-            for directional in self.directionals:
-                diffuseLight, specularLight = directional(
-                    diffuseLight, specularLight, mesh.vertex_normals, mesh.vertices, eyes,
-                    mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
-            if mesh.textures.dim() == 4:
-                mesh.textures = torch.clamp(mesh.textures * diffuseLight[:, :, None, :] +
-                                            torch.ones_like(mesh.textures) * specularLight[:, :, None, :], 0.0, 1.0)
-            elif mesh.textures.dim() == 6:
-                mesh.textures = torch.clamp(mesh.textures * diffuseLight[:, :, None, None, None, :] +
-                                            torch.ones_like(mesh.textures) * specularLight[:, :, None, None, None, :], 0.0, 1.0)
-        return mesh
+        elif per_face:
+            diffuseLight = torch.zeros(mesh.faces.shape, dtype=torch.float32, device=mesh.vertices.device)
+        else:
+            diffuseLight = torch.zeros(mesh.textures.shape, dtype=mesh.textures.dtype, device=mesh.vertices.device)
+        specularLight = torch.zeros_like(diffuseLight)
+        diffuseLight = self.ambient(diffuseLight)
+        for directional in self.directionals:
+            diffuseLight, specularLight = self._directional(directional, diffuseLight, specularLight, mesh, eyes)
+        if per_face:
+            return diffuseLight[:, :, None, :], specularLight[:, :, None, :]
+        return diffuseLight, specularLight
+
+    def _compose(self, mesh, diffuseLight, specularLight):
+        """lighting.py:196-220: clamp(SSS(diffuse, specular, mesh), 0, 1) for a surface mesh with with_SSS and 4-D
+        textures, else clamp(textures * diffuse + specular, 0, 1) on 4-D or 6-D textures, the vertex, face or texel
+        terms broadcast over the texel dimensions."""
+        tx = mesh.textures
+        if self.light_mode == 'surface' and mesh.with_SSS and tx.dim() == 4:
+            return torch.clamp(SSS(diffuseLight, specularLight, mesh, grad=self.sss_grad), 0.0, 1.0)
+        if tx.dim() not in (4, 6):
+            # The reference only applies vertex lighting to 4-D / 6-D textures (lighting.py:214-220);
+            # the documented vertex texture shape [B, nv, 3] therefore passes through unlit.
+            return tx
+        texels = (Ellipsis,) + (None,) * (tx.dim() - diffuseLight.dim()) + (slice(None),)
+        return torch.clamp(tx * diffuseLight[texels] + torch.ones_like(tx) * specularLight[texels], 0.0, 1.0)
 
     def forward(self, mesh, eyes=None):
         if self.Gbuffer == "albedo":
             return mesh
-        if self.Gbuffer in GBUFFER_MODES:
-            return self._gbuffer(mesh, eyes)
-        if self.light_mode == 'surface' and mesh.with_SSS and mesh.textures.dim() == 4:
-            return self._subsurface(mesh, eyes)
-        if self.light_mode == 'surface' and mesh.normal_textures is not None:
-            return self._normal_mapped(mesh, eyes)
-        if self.light_mode == 'surface' and self._fusable(mesh, eyes):
-            lit = self._fused_surface(mesh, eyes)
+        surface = self.light_mode == 'surface'
+        if surface and mesh.normal_textures is not None:
+            self._check_normal_map(mesh)
+        if surface and not (mesh.with_SSS and mesh.textures.dim() == 4):
+            lit = self._fused(mesh, eyes)
             if lit is not None:
                 mesh.textures = lit
                 return mesh
-        if self.light_mode == 'surface':
-            diffuseLight = torch.zeros(mesh.faces.shape, dtype=torch.float32, device=mesh.vertices.device)
-            specularLight = torch.zeros_like(diffuseLight)
-            diffuseLight = self.ambient(diffuseLight)
-            for directional in self.directionals:
-                diffuseLight, specularLight = directional(
-                    diffuseLight, specularLight, mesh.surface_normals, torch.sum(mesh.face_vertices, dim=2) / 3.0, eyes,
-                    mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
-            diffuseLight = diffuseLight[:, :, None, :]
-            specularLight = specularLight[:, :, None, :]
-            if mesh.textures.dim() == 4:
-                mesh.textures = torch.clamp(mesh.textures * diffuseLight + torch.ones_like(mesh.textures) * specularLight, 0.0, 1.0)
-            elif mesh.textures.dim() == 6:
-                mesh.textures = torch.clamp(mesh.textures * diffuseLight[:, :, :, None, None, :] +
-                                            torch.ones_like(mesh.textures) * specularLight[:, :, :, None, None, :], 0.0, 1.0)
-        elif self.light_mode == 'vertex':
-            diffuseLight = torch.zeros(mesh.vertices.shape, dtype=torch.float32, device=mesh.vertices.device)
-            specularLight = torch.zeros_like(diffuseLight)
-            diffuseLight = self.ambient(diffuseLight)
-            for directional in self.directionals:
-                diffuseLight, specularLight = directional(
-                    diffuseLight, specularLight, mesh.vertex_normals, mesh.vertices, eyes,
-                    mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
-            # The reference only applies vertex lighting to 4-D / 6-D textures (lighting.py:214-220);
-            # the documented vertex texture shape [B, nv, 3] therefore passes through unlit.
-            if mesh.textures.dim() == 4:
-                mesh.textures = torch.clamp(mesh.textures * diffuseLight[:, :, None, :] +
-                                            torch.ones_like(mesh.textures) * specularLight[:, :, None, :], 0.0, 1.0)
-            elif mesh.textures.dim() == 6:
-                mesh.textures = torch.clamp(mesh.textures * diffuseLight[:, :, None, None, None, :] +
-                                            torch.ones_like(mesh.textures) * specularLight[:, :, None, None, None, :], 0.0, 1.0)
+        if self.Gbuffer in GBUFFER_MODES:   # directional_lighting.py:136-144 replaces the light terms; ones take them
+            mesh.textures = torch.ones_like(mesh.textures)
+        mesh.textures = self._compose(mesh, *self._light_terms(mesh, eyes))
         return mesh
 
     execute = forward

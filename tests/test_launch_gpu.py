@@ -99,3 +99,46 @@ def test_softras_forward_backward_launches_seven_kernels(cuda_device):
     delta, counts = profiled(L, softras, cuda_device)
     assert delta == 7
     assert [counts[k] for k in (0, 20, 1, 4, 2, 3, 9)] == [1] * 7, counts
+
+
+ROUTES = ("_fused_surface", "_fused_normal_mapped", "_fused_gbuffer", "_fused_normal_mapped_gbuffer")
+
+
+@pytest.mark.parametrize("route,gbuffer,kernel,launches", [
+    ("_fused_surface", 'None', "_FusedSurfaceLighting", 1),
+    ("_fused_normal_mapped", 'None', "_FusedNormalMappedLighting", 1),
+    ("_fused_gbuffer", 'normal', "_FusedGbuffer", 1),
+    ("_fused_gbuffer", 'depth', "_FusedGbuffer", 2),   # the depth pass, then the G-buffer
+    ("_fused_normal_mapped_gbuffer", 'normal', "_FusedNormalMappedGbuffer", 1)])
+def test_each_fused_lighting_route_launches_its_kernel(cuda_device, route, gbuffer, kernel, launches):
+    """Lighting's fused dispatcher on each kernel's route: asked by that route's name it returns the kernel's result,
+    from `launches` forward and as many backward launches, all under B200R_K_LIGHTING; the other routes' names
+    return None on the same inputs."""
+    from jrender_b200 import lighting
+    dev = cuda_device
+    v, f = wl.sphere_by_faces(280)
+    nf = f.shape[0]
+    g = torch.Generator().manual_seed(0)
+    kw = {}
+    if "normal_mapped" in route:
+        n = torch.nn.functional.normalize(torch.rand(1, nf, 4, 3, generator=g) - 0.5 + torch.tensor([0., 0., 1.]), dim=3)
+        tbn = torch.eye(3)[None, None].repeat(1, nf, 1, 1) + 0.1 * torch.rand(1, nf, 3, 3, generator=g)
+        kw = dict(normal_textures=n.to(dev).requires_grad_(True), TBN=tbn.to(dev))
+    m = jr.Mesh(torch.from_numpy(v)[None].to(dev).requires_grad_(True), torch.from_numpy(f)[None].to(dev),
+                textures=torch.rand(1, nf, 4, 3, generator=g).to(dev).requires_grad_(True), texture_res=2, **kw)
+    eyes = torch.tensor([[0.3, 0.4, -2.5]], device=dev)
+    tr = jr.Transform(camera_mode='look_at')
+    tr.set_eyes(eyes)
+    light = jr.Lighting(Gbuffer=gbuffer, transform=tr)
+    for other in ROUTES:
+        if other != route:
+            assert getattr(light, other)(m, eyes) is None, other
+    L = _lib.lib()
+    out = []
+    fwd = lambda dev: out.append(getattr(light, route)(m, eyes))
+    fwd(dev)                               # warm up
+    delta, counts = profiled(L, fwd, dev)
+    assert out[-1] is not None and type(out[-1].grad_fn)._forward_cls is getattr(lighting, kernel)
+    assert delta == counts[15] == sum(counts) == launches, (delta, counts)   # B200R_K_LIGHTING
+    delta, counts = profiled(L, lambda dev: out[-1].sum().backward(), dev)
+    assert delta == counts[15] == sum(counts) == launches, (delta, counts)

@@ -89,23 +89,9 @@ def main():
             return light(mesh, eye).textures
 
     def terms():
-        """The op-by-op diffuse / specular light of Lighting._subsurface, without SSS."""
+        """The op-by-op diffuse / specular light of Lighting, without SSS."""
         with torch.no_grad():
-            if mesh.normal_textures is not None:
-                d = torch.zeros(textures.shape, device=dev)
-                s = torch.zeros_like(d)
-                d = light.ambient(d)
-                dl = light.directionals[0]
-                return lighting.directional_lighting_texels(d, s, mesh.surface_ResNormals, dl.light_intensity,
-                                                            dl.light_color, dl.light_direction,
-                                                            torch.sum(mesh.face_vertices, dim=2) / 3.0, eye,
-                                                            mesh.with_specular, mesh.metallic_textures,
-                                                            mesh.roughness_textures)
-            d = torch.zeros(mesh.faces.shape, device=dev)
-            s = torch.zeros_like(d)
-            d = light.ambient(d)
-            return light.directionals[0](d, s, mesh.surface_normals, torch.sum(mesh.face_vertices, dim=2) / 3.0, eye,
-                                         mesh.with_specular, mesh.metallic_textures, mesh.roughness_textures)
+            return light._light_terms(mesh, eye)
 
     ms, mn = timed(frame, a.iters, a.rounds)
     print(json.dumps(dict(what="SSS frame (Lighting with with_SSS)", ms_median=ms, ms_min=mn, rounds=a.rounds,
