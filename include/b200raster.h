@@ -460,6 +460,28 @@ B200R_API int b200r_sss_blur_pyramid_backward(const float* stretch_u, const floa
                                               size_t workspace_bytes, const float* taps, const float* tap_widths,
                                               const float* weights, int num_levels, int height, int width, void* stream);
 
+/* ---- screen-space image passes (render2) --------------------------------------------------------------------------
+ * Replace SSAO_cuda, SSDO_cuda and FXAA_cuda (jrender/render2/utils/cuda/{SSAO,SSDO,FXAA}_cuda.py).  Images are square,
+ * image_size x image_size pixels, HWC, row 0 at the top; 1 <= image_size and 3 * image_size^2 <= INT_MAX.  One launch
+ * each; no gradients.
+ *   b200r_ssao: depth [is, is] (view-space z), face_ind [is, is] int32 (-1 = background), normals [is, is, 3] (view
+ *       space) -> occlusion [is, is]: for each covered pixel, the share of sample_num points drawn in a half ball of radius
+ *       sample_range_r around the pixel's view-space point (x, y = NDC * width * z) whose projection lands on a pixel in
+ *       front of it; 0 on the background.  Pixel i draws from curand XORWOW curand_init(1, i, 0), x, y, z per sample,
+ *       as the reference does, so the results are the reference's bit for bit.  sample_num >= 0 (0 gives NaN).
+ *   b200r_ssdo: the same samples; color [is, is, 3] -> image [is, is, 3]: the ambient share (samples whose pixel is no
+ *       more than 0.01 in front of them) times the colour, plus one bounce of indirect light from the other samples'
+ *       pixels; the background passes the colour through.
+ *   b200r_fxaa: texture [is, is, 3] -> image [is, is, 3], the reference's FXAA: its edge search never moves (see
+ *       DESIGN.md), so a pixel is either kept or resampled bilinearly at the sub-pixel offset across its edge.  Reads only
+ *       inside the image; the taps the reference reads past the last row count as 0, as they have weight 0 there.
+ * The three launches are profiled under B200R_K_SSS, the id of the image passes. */
+B200R_API int b200r_ssao(const float* depth, const int32_t* face_ind, const float* normals, float* occlusion,
+                         int image_size, int sample_num, float sample_range_r, float width, void* stream);
+B200R_API int b200r_ssdo(const float* color, const float* depth, const int32_t* face_ind, const float* normals,
+                         float* image, int image_size, int sample_num, float sample_range_r, float width, void* stream);
+B200R_API int b200r_fxaa(const float* texture, float* image, int image_size, void* stream);
+
 /* Launch counter: number of kernels this library has launched in this process
  * (bench.py reports the delta over the timed region as "gpu_launches"). */
 B200R_API unsigned long long b200r_launch_count(void);
