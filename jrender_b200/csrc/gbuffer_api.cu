@@ -84,8 +84,13 @@ __device__ __forceinline__ float camera_depth(const GbArgs& A, const b200r_camer
     return cam[2];
 }
 
-// numpy's max: NaN as soon as either is NaN
-__device__ __forceinline__ float nan_max(float a, float b) { return a != a ? a : (b != b ? b : (b > a ? b : a)); }
+// numpy's max: NaN as soon as either is NaN; between the two zeros +0 > -0 (IEEE 754-2019 maximum), so the sign of a
+// zero max, and with it the sign of every z / M, does not depend on which face the fold reaches first
+__device__ __forceinline__ float nan_max(float a, float b) {
+    if (a != a) return a;
+    if (b != b) return b;
+    return (b > a || (b == a && signbit(a) && !signbit(b))) ? b : a;
+}
 
 // Every thread of the block gets the fold of its threads' x: max (MAX) or sum, in one fixed tree order.
 template <bool MAX>

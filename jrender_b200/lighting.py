@@ -162,13 +162,15 @@ GBUFFER_MODES = ('normal', 'depth')
 
 
 class _TiedMax(torch.autograd.Function):
-    """max over every element of x, NaN if any is NaN (numpy's max, as the reference's jt.max is read here).  The
-    gradient goes in full to every element equal to the max -- Jittor's reduce-max gradient, the mask x == max -- not
-    split over ties as torch.max's is."""
+    """max over every element of x, NaN if any is NaN (numpy's max, as the reference's jt.max is read here), and +0
+    when both zeros reach a zero max (IEEE 754-2019 maximum: +0 > -0; the reference's own rule is not known, this is
+    the port's, and the depth kernel's).  The gradient goes in full to every element equal to the max -- Jittor's
+    reduce-max gradient, the mask x == max -- not split over ties as torch.max's is."""
 
     @staticmethod
     def forward(ctx, x):
         m = x.max()
+        m = torch.where((m == 0) & ((x == 0) & ~torch.signbit(x)).any(), torch.zeros_like(m), m)
         ctx.save_for_backward(x, m)
         return m
 

@@ -205,11 +205,35 @@ def _normal_f64(v, lift, c):
     return Nval, Njac, n32, EV(ln, le)
 
 
+def normal_duals(w, c, vl, Nval, Njac, n32, ln, lift):
+    """normal_duals: the corners as Dual<9> variables dv, and the normal Nd with value Nval and partials of the float32
+    cross product's duals through (I - N N^T) / |c| (Njac for N, n32 for |c|), or I / 1e-12 on normalize's eps path
+    (decided on ln, the unclamped norm).  Returns (dv, Nd)."""
+    zero = full(vl[0], 0)
+    one = zero + c(1.0)
+    dv = [Dual(vl[k], [one if j == k else zero for j in range(9)]) for k in range(9)]
+    ae = [dv[0] - dv[3], dv[1] - dv[4], dv[2] - dv[5]]
+    be = [dv[6] - dv[3], dv[7] - dv[4], dv[8] - dv[5]]
+    cr = [be[1] * ae[2] - be[2] * ae[1], be[2] * ae[0] - be[0] * ae[2], be[0] * ae[1] - be[1] * ae[0]]
+    inv = c(1.0) / n32
+    st = w.decide("norm_eps", ln, np.float64(1e-12) if lift is None else EV(1e-12),
+                  lambda x, lo: np.where(np.asarray(x) >= lo, 1, 0).astype(np.int8))
+    on_eps = st != 1
+    Nd = []
+    for j in range(3):
+        parts = []
+        for k in range(9):
+            Ndc = where(on_eps, zero, (Njac[0] * cr[0].d[k] + Njac[1] * cr[1].d[k]) + Njac[2] * cr[2].d[k])
+            parts.append((cr[j].d[k] - Njac[j] * Ndc) * inv)
+        Nd.append(Dual(Nval[j], parts))
+    return dv, Nd
+
+
 def _gather_vertices(a, b, f):
     """The three corners of faces f of batch elements b, [n, 9] float32, and their vertex indices [n, 3]."""
     fi = a["faces"][np.where(a["Bf"] == 1, 0, b), f]
-    vb = a["vertices"][np.where(a["Bv"] == 1, 0, b)]
-    v = np.concatenate([vb[np.arange(len(b)), fi[:, k]] for k in range(3)], axis=1)
+    bv = np.broadcast_to(np.where(a["Bv"] == 1, 0, b), np.shape(b))
+    v = np.concatenate([a["vertices"][bv, fi[:, k]] for k in range(3)], axis=1)
     return v, fi
 
 
@@ -323,23 +347,7 @@ def surface_backward(a, lift=None, replay=None):
             out["metallic"].append(gm)
             out["roughness"].append(gr)
         if want_v:
-            zero = full(vl[0], 0)
-            one = zero + c(1.0)
-            dv = [Dual(vl[k], [one if j == k else zero for j in range(9)]) for k in range(9)]
-            ae = [dv[0] - dv[3], dv[1] - dv[4], dv[2] - dv[5]]
-            be = [dv[6] - dv[3], dv[7] - dv[4], dv[8] - dv[5]]
-            cr = [be[1] * ae[2] - be[2] * ae[1], be[2] * ae[0] - be[0] * ae[2], be[0] * ae[1] - be[1] * ae[0]]
-            inv = c(1.0) / n32
-            st = w.decide("norm_eps", ln, np.float64(1e-12) if lift is None else EV(1e-12),
-                          lambda x, lo: np.where(np.asarray(x) >= lo, 1, 0).astype(np.int8))
-            on_eps = st != 1
-            Nd = []
-            for j in range(3):
-                parts = []
-                for k in range(9):
-                    Ndc = where(on_eps, zero, (Njac[0] * cr[0].d[k] + Njac[1] * cr[1].d[k]) + Njac[2] * cr[2].d[k])
-                    parts.append((cr[j].d[k] - Njac[j] * Ndc) * inv)
-                Nd.append(Dual(Nval[j], parts))
+            dv, Nd = normal_duals(w, c, vl, Nval, Njac, n32, ln, lift)
             pd = [((dv[k] + dv[3 + k]) + dv[6 + k]) / c(3.0) for k in range(3)]
             dd, sd = face_light(w, c, Nd, pd, L, ey if spec else None, m, r)
             terms = []

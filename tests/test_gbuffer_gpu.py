@@ -1,12 +1,16 @@
 """The G-buffer kernels (csrc/gbuffer_api.cu) on the GPU.
 
-Forward: every recorded kernel call (kernel_calls fixture) bit for bit against oracle/gbuffer.py's float32 emulation,
-with the same NaN / +-inf pattern.  Gradients: against float64 autograd of the op-by-op mirror (Lighting.fused = False on
-the CPU) within 1e-4 of each gradient's max |finite value|, with the same non-finite pattern, on the edge scenes of
-tests/gbuffer_edge_cases.py.  End to end: Renderer(Gbuffer=...) images against the reference pipeline's
-(tests/golden/ref_host_gbuffer.npz), within 1e-3 of the max for SoftRas and 1e-4 for NMR.
-Launches: at most two forward and two backward.  CUDA graphs: a depth-mode render and
-its backward captured and replayed give the eager images bit for bit.
+Every recorded kernel call (kernel_calls fixture), forward and backward, against oracle/gbuffer.py's float32 emulation
+(hold_to_emulation): bit for bit, with the same NaN / +-inf pattern, the G-buffer, the depth workspace's used prefix
+(face_z and the partial maxima after the forward, face_G and the partial sums after the backward), depth_max with its
+sign, and grad_metallic, grad_roughness and grad_normal_textures; each grad_vertices entry within term_sums' bound of
+the exact sum of the emulated terms of both depth kernels, gamma_{n-1} sum |t| for its n float atomics
+(oracle/preraster.py).  The emulation itself is held to float64 autograd entry by entry in tests/test_gbuffer_cpu.py.
+Coarser, end to end, on the edge scenes of tests/gbuffer_edge_cases.py: the G-buffer against the op-by-op float64 mirror
+within 2e-5, and the gradients against its autograd within 1e-4 of each gradient's max |finite value|, with the same
+non-finite pattern (normal-mode slivers, for which no fixed bound holds, are held to the emulation alone).  Renderer(Gbuffer=...) images against the reference pipeline's (tests/golden/ref_host_gbuffer.npz),
+within 1e-3 of the max for SoftRas and 1e-4 for NMR.  Launches: at most two forward and two backward.  CUDA graphs: a
+depth-mode render and its backward captured and replayed give the eager images bit for bit.
 """
 import os
 
@@ -18,6 +22,7 @@ import jrender_b200 as jr
 from jrender_b200 import _lib
 from jrender_b200 import workloads as wl
 from oracle import gbuffer as OG
+from oracle.preraster import term_sums
 from tests import gbuffer_edge_cases as E
 
 pytestmark = pytest.mark.gpu
@@ -27,7 +32,8 @@ G = os.path.join(os.path.dirname(__file__), "golden", "ref_host_gbuffer.npz")
 
 @pytest.fixture
 def kernel_calls(monkeypatch):
-    """Every call of the four G-buffer entry points made while the test runs: (name, arguments after the call)."""
+    """Every call of the four G-buffer entry points made while the test runs: (name, oracle.gbuffer.args_from_call of
+    its arguments after the call)."""
     calls = []
     real = _lib.call
 
@@ -35,7 +41,7 @@ def kernel_calls(monkeypatch):
         real(name, device, *args)
         if name in OG.CALLS:
             torch.cuda.synchronize(device)
-            calls.append((name, OG.args_from_call(name, args) if "forward" in name else None))
+            calls.append((name, OG.args_from_call(name, args)))
     monkeypatch.setattr(_lib, "call", record)
     return calls
 
@@ -48,20 +54,61 @@ def _same_bits(got, want, what):
         what, bad.sum(), bad.size, np.argwhere(bad)[0], got[bad][0], want[bad][0])
 
 
-def _hold_forward(calls):
-    n = 0
+def _same_signed(got, want, what):
+    """Equal bits, NaN for NaN: unlike ==, tells +0 from -0."""
+    got, want = np.asarray(got, np.float32).reshape(-1), np.asarray(want, np.float32).reshape(-1)
+    same = (got.view(np.int32) == want.view(np.int32)) | (np.isnan(got) & np.isnan(want))
+    assert same.all(), "%s: %r vs %r" % (what, got[~same], want[~same])
+
+
+def _hold_vertices(name, gv, emu):
+    t = np.asarray(emu["vertex_terms"], np.float32).reshape(-1)
+    sl = np.asarray(emu["vertex_slots"]).reshape(-1)
+    live = t != 0   # the kernels skip zero terms
+    s = term_sums(sl[live], t[live], gv.size)
+    got = gv.reshape(-1).astype(np.float64)
+    fin = np.isfinite(s["exact"])
+    _same_bits(np.where(fin, 0, got).astype(np.float32), np.where(fin, 0, s["exact"]).astype(np.float32),
+               name + " grad_vertices non-finite entries")
+    err = np.abs(got - s["exact"])[fin]
+    ratio = err / np.maximum(s["bound"][fin], 1e-300)
+    assert (err <= s["bound"][fin]).all(), (name, "grad_vertices", ratio.max())
+    return float(ratio.max(initial=0.0))
+
+
+def hold_to_emulation(calls):
+    """Each recorded call against oracle.gbuffer's emulation of it (module docstring).  Returns the number of backward
+    calls checked."""
+    assert calls, "no G-buffer kernel ran"
+    nb, worst = 0, 0.0
     for name, a in calls:
-        if a is None:
-            continue
-        if name == "b200r_gbuffer_lighting_forward":
+        nm = name in OG.NM_PTRS
+        if name.endswith("_forward"):
+            if nm:
+                _same_bits(a["out"], OG.nm_gbuffer_forward(a), name)
+                continue
             want, M = OG.gbuffer_forward(a)
             _same_bits(a["out"].reshape(want.shape), want, name)
             if M is not None:
-                _same_bits(a["depth_max"], [M], name + " depth_max")
-        else:
-            _same_bits(a["out"], OG.nm_gbuffer_forward(a), name)
-        n += 1
-    return n
+                n = a["B"] * a["nf"]
+                z, partials, _ = OG.face_depths(a)
+                _same_bits(a["workspace"][:n], z, name + " face_z")
+                _same_bits(a["workspace"][n:n + len(partials)], partials, name + " max partials")
+                _same_signed(a["depth_max"], [M], name + " depth_max")
+            continue
+        emu = (OG.nm_gbuffer_backward if nm else OG.gbuffer_backward)(a)
+        for k in ("normal_textures", "metallic", "roughness"):
+            if a.get("grad_" + k) is not None:
+                _same_bits(a["grad_" + k], emu[k], "%s grad_%s" % (name, k))
+        if not nm and a["mode"] == 1:
+            n = a["B"] * a["nf"]
+            _same_bits(a["workspace"][:n], emu["face_G"], name + " face_G")
+            _same_bits(a["workspace"][n:n + len(emu["partials"])], emu["partials"], name + " sum partials")
+        if a.get("grad_vertices") is not None:
+            worst = max(worst, _hold_vertices(name, a["grad_vertices"], emu))
+        nb += 1
+    print("grad_vertices: worst |kernel - exact sum of emulated terms| / bound = %.3g" % worst)
+    return nb
 
 
 def _close_grad(got, want, what):
@@ -80,8 +127,8 @@ def _close_grad(got, want, what):
 def test_kernels_against_emulation_and_float64_mirror(name, kernel_calls):
     sc = E.scene(name)
     out, grads = E.run(sc, torch.device("cuda"), torch.float32, fused=True)
-    assert {n for n, _ in kernel_calls} >= E.expected_calls(sc)
-    assert _hold_forward(kernel_calls) >= 1
+    assert {n for n, _ in kernel_calls} == E.expected_calls(sc)
+    assert hold_to_emulation(kernel_calls) == 1
     ref_out, ref_grads = E.run(sc, torch.device("cpu"), torch.float64, fused=False)
     assert np.array_equal(np.isnan(out), np.isnan(ref_out)), name
     fin = np.isfinite(ref_out)
@@ -89,18 +136,19 @@ def test_kernels_against_emulation_and_float64_mirror(name, kernel_calls):
     for k, g in ref_grads.items():
         if g is None:
             assert grads[k] is None, (name, k)
-        elif any(t in name for t in ("_metallic_", "_roughness_")):
-            # Known difference at a non-finite material input: the kernels' forward-mode duals multiply a zero tangent
-            # by the non-finite value (0 * NaN), where the mirror's reverse mode never forms that product, so the
-            # kernel's gradient may be NaN where the mirror's is finite.  It is NaN wherever the mirror's is, and
-            # within the bound wherever both are finite.
-            got = np.asarray(grads[k], np.float64)
-            assert np.isnan(got[np.isnan(g)]).all(), (name, k)
-            fin = np.isfinite(got) & np.isfinite(g)
-            scale = max(np.abs(g[np.isfinite(g)]).max(initial=0), 1e-30)
-            assert np.abs(got[fin] - g[fin]).max(initial=0) <= GRAD_TOL * scale, (name, k)
-        else:
+        elif not any(t in name for t in ("_metallic_", "_roughness_")):
+            # At a non-finite material input the kernels' forward-mode duals form 0 * NaN where the mirror's reverse
+            # mode never does: there the gradients are held to the emulation above alone, which forms it too.
             _close_grad(grads[k], g, "%s: grad %s" % (name, k))
+
+
+@pytest.mark.parametrize("name", E.SLIVER_NORMAL)
+def test_normal_slivers_against_emulation(name, kernel_calls):
+    """Normal-mode slivers, with and without the specular branch: no fixed bound against the float64 mirror holds for
+    their normals (tests/gbuffer_edge_cases.py), so every call is held to the emulation, which
+    tests/test_gbuffer_cpu.py holds to float64 autograd per entry."""
+    E.run(E.scene(name), torch.device("cuda"), torch.float32, fused=True)
+    assert hold_to_emulation(kernel_calls) == 1
 
 
 def test_head_sized_normal_map_against_float64_mirror():
